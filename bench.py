@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py — train tokens/s of a Llama-2-7B NF4+double-quant LoRA finetuning step (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # our arm (fused sm_100a Linear4bit), 1 process / GPU
+  python bench.py --gpus N --steps K --warmup W            # our arm (fused sm_90a Linear4bit), 1 process / GPU
+  python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed, as DIR/*.npy
   python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle dequant + CPU matmul)
   python bench.py --impl unfused ...                       # bnb-equivalent GPU restatement (dequant kernel + cuBLAS)
 
@@ -52,14 +53,17 @@ def parse_args():
                          "flat adapter buffer; torch = torch.optim.AdamW(fused, capturable)")
     ap.add_argument("--buckets", type=int, default=1,
                     help="gradient allreduce buckets; > 1 = reverse-layer buckets overlapped with backward on a side stream (DDP's scheme). "
-                         "Measured slower than one allreduce after backward at 2 GPUs (96.7 vs 95.3 ms): the NCCL kernels take SMs from "
-                         "the persistent NF4 kernel, whose static schedule then needs a second round — see DESIGN.md 5")
+                         "The NCCL kernels take SMs from the persistent NF4 kernel, whose static schedule then needs a second round — "
+                         "see DESIGN.md 5")
     ap.add_argument("--cpu-reps", type=int, default=3, help="repetitions of the CPU sample (median reported)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (loss, a fixed sample of the LoRA gradients and "
+                         "updated adapter weights) as DIR/<name>.npy, to compare two builds output for output")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------
-# clocks sampling during the timed region (B200_PROFILING.md "clocks line")
+# clocks sampling during the timed region (SM clock, power cap and throttle reasons beside the number)
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
     QUERY = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -249,8 +253,16 @@ def run_reference_arm(args):
 # GPU arms
 # ---------------------------------------------------------------------------------------------
 def run_gpu_arm(args):
+    # The same arguments must give the same outputs every run (--dump-outputs compares builds output for output): every
+    # kernel of the step runs in its deterministic form, or the run stops with the name of the op that has none.  Flash
+    # attention's backward otherwise accumulates dQ with atomics; cuBLAS needs a fixed workspace configuration, which it
+    # reads when its first handle is created.
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
     import torch
     import torch.distributed as dist
+
+    torch.use_deterministic_algorithms(True)
+    torch.utils.deterministic.fill_uninitialized_memory = False   # every output buffer is written in full; no fill kernels
 
     import qlora_b200 as q
     import harness.llama_qlora as H
@@ -423,6 +435,8 @@ def run_gpu_arm(args):
         sampler.start()
     QF.LAUNCH_COUNTER[0] = 0
     t_res = timed(loop_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, static_loss, gsync, params)
     if graphs:
         launches = args.steps * sum(launches_per_kind[kind_of(mi)] for mi in range(accum))
     else:
@@ -450,7 +464,6 @@ def run_gpu_arm(args):
             d[0] += 1
             d[1] += ms
             d[2] += 2.0 * m * n * k
-        log_copy = list(QF.EVENT_LOG)
         QF.EVENT_LOG = None
         peaks = {}
         try:
@@ -458,28 +471,11 @@ def run_gpu_arm(args):
         except Exception:
             pass
         peak = peaks.get("bf16_tflops_sustained")
-        peak_src = "measured sustained (MEASURED_PEAKS.json)" if peak else "fallback (B200_PROFILING.md, sustained)"
-        peak = peak or 1400.0
+        peak_src = "measured sustained (MEASURED_PEAKS.json)" if peak else "H100 SXM data sheet, dense bf16 at 700 W (not reached)"
+        peak = peak or 989.0
         achieved = tot_flops / (tot_ms * 1e-3) / 1e12 if tot_ms > 0 else 0.0
-        # DRAM traffic per launch: launch-mix average of the ncu-measured bytes per launch kind — profiles/r2_traffic_by_kind.json
-        traffic, traffic_src = None, None
-        try:
-            tb = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic_by_kind.json")))
-            tot_b, ok = 0.0, bool(log_copy)
-            for kind, m, n, k, _e0, _e1 in log_copy:
-                key = f"{kind}:{n}x{k}:M{m}"
-                if key not in tb["bytes"]:
-                    ok = False
-                    break
-                tot_b += tb["bytes"][key]
-            if ok:
-                traffic = tot_b / len(log_copy)
-                traffic_src = "launch-mix mean of dram__bytes_read+write per launch, ncu --set full (profiles/r2_traffic_by_kind.json)"
-        except Exception:
-            pass
-        roof = {"bound": "tensor", "kernel": "nf4_gemm_pair_kernel (fused NF4 dequant + tcgen05 GEMM + LoRA step; grouped q/k/v and gate/up, fwd + dX)",
-                "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
-                "traffic_unit": "bytes/launch", "traffic_source": traffic_src, "peak_source": peak_src,
+        roof = {"bound": "tensor", "kernel": "nf4_gemm_wgmma_kernel (fused NF4 dequant + wgmma GEMM + LoRA step; grouped q/k/v and gate/up, fwd + dX)",
+                "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "peak_source": peak_src,
                 "launches_timed": n_l, "avg_launch_us": 1e3 * tot_ms / max(n_l, 1),
                 "by_kind": {kk: {"launches": v[0], "avg_us": 1e3 * v[1] / v[0], "tflops": v[2] / (v[1] * 1e-3) / 1e12} for kk, v in by_kind.items()}}
 
@@ -568,6 +564,26 @@ def run_gpu_arm(args):
                                     "sample": ref.describe(len(ts)), "t_layer_s": {"median": t_layer, "min": min(ts), "max": max(ts)}}
         emit(line)
     teardown(graphs, world)
+
+
+DUMP_SAMPLE = 1 << 22   # elements sampled from each adapter-sized output (16 MB of float32)
+
+
+def dump_outputs(out_dir, loss, gsync, params):
+    """What the last timed step handed back to the training loop: the loss, the LoRA gradients and the adapter weights after
+    the optimizer step.  The two adapter-sized arrays are sampled at the same fixed, seeded positions every run."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    weights = gsync.flat_param if gsync.flat_param is not None else torch.cat([p.detach().reshape(-1) for p in params])
+    n = gsync.flat.numel()
+    idx = np.unique(np.random.default_rng(20240611).integers(0, n, size=min(n, DUMP_SAMPLE)))
+    idx_d = torch.from_numpy(idx).to(gsync.flat.device)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().cpu().numpy().reshape(1))
+    np.save(os.path.join(out_dir, "lora_grad_sample.npy"), gsync.flat[idx_d].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "lora_weight_sample.npy"), weights[idx_d].float().cpu().numpy())
 
 
 def teardown(graphs, world):

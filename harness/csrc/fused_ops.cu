@@ -3,7 +3,7 @@
 //   hops_rope_qk   : RoPE (HF rotate_half form) on q and k in one launch; backward = same kernel with sign = -1
 //   hops_swiglu_fwd: silu(gate) * up
 //   hops_swiglu_bwd: d_gate, d_up from (gate, up, d_out)
-// bf16 in / bf16 out, fp32 math, 16 B vector accesses.  sm_100a.
+// bf16 in / bf16 out, fp32 math, 16 B vector accesses.  sm_90a.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -300,9 +300,16 @@ __global__ void __launch_bounds__(256) dropout_kernel(const uint4* __restrict__ 
   }
 }
 
+int sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
+    n = 132;
+  return n;
+}
+
 unsigned grid_for(int64_t n) {
   int64_t b = (n + 255) / 256;
-  const int64_t cap = 148LL * 16;
+  static const int64_t cap = int64_t(sm_count()) * 16;   // grid-stride beyond 16 CTAs per SM
   return unsigned(b > cap ? cap : (b < 1 ? 1 : b));
 }
 

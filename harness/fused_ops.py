@@ -20,7 +20,7 @@ def build(force: bool = False) -> str:
     if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= os.path.getmtime(_SRC):
         return LIB_PATH
     nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+    subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
                     "-shared", "-o", LIB_PATH + ".tmp", _SRC, "-cudart", "static"], check=True)
     os.replace(LIB_PATH + ".tmp", LIB_PATH)
     return LIB_PATH

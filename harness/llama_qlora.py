@@ -85,12 +85,12 @@ class LoRALinear4bit(nn.Module):
 
     _next_salt = [1]
 
-    def __init__(self, base, r: int, alpha: int, dropout: float, device=None, seed_tensor=None):
+    def __init__(self, base, r: int, alpha: int, dropout: float, device=None, seed_tensor=None, generator=None):
         super().__init__()
         self.base_layer = base
         self.lora_A = nn.Linear(base.in_features, r, bias=False, dtype=torch.bfloat16, device=device)
         self.lora_B = nn.Linear(r, base.out_features, bias=False, dtype=torch.bfloat16, device=device)
-        nn.init.kaiming_uniform_(self.lora_A.weight, a=math.sqrt(5))
+        nn.init.kaiming_uniform_(self.lora_A.weight, a=math.sqrt(5), generator=generator)
         nn.init.zeros_(self.lora_B.weight)
         self.scaling = alpha / r
         self.p = float(dropout)
@@ -243,8 +243,9 @@ class LlamaQLoRA(nn.Module):
         self.norm = RMSNorm(shape.hidden, shape.rms_eps, device)
         self.lm_head = nn.Linear(shape.hidden, shape.vocab, bias=False, device=device, dtype=torch.bfloat16)
         self.lm_head.weight.requires_grad_(False)
-        nn.init.normal_(self.embed_tokens.weight, std=0.02)
-        nn.init.normal_(self.lm_head.weight, std=0.02)
+        # every initial value comes from `gen`: the same seed builds the same model in every run
+        nn.init.normal_(self.embed_tokens.weight, std=0.02, generator=gen)
+        nn.init.normal_(self.lm_head.weight, std=0.02, generator=gen)
         self._rope_cache = {}
         # data parallel: called with i when the backward of decoder layer i has been enqueued (harness/dp.py starts the
         # allreduce of the gradient buckets that layer completes)
@@ -272,7 +273,8 @@ class LlamaQLoRA(nn.Module):
             assert sorted(targets) == sorted(leaf_names), targets
             for layer in self.layers:
                 for name in targets:
-                    setattr(layer, name, LoRALinear4bit(getattr(layer, name), lora_r, lora_alpha, lora_dropout, device, self.dropout_seed))
+                    setattr(layer, name, LoRALinear4bit(getattr(layer, name), lora_r, lora_alpha, lora_dropout, device, self.dropout_seed,
+                                                          generator=gen))
                 # adapters that are used together live side by side: lora_A of q/k/v (gate/up) are row blocks of ONE buffer, so
                 # the grouped launch's batched projection x . [A_q; A_k; A_v]^T needs no concatenation (same values, same init)
                 for grp in (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj")):

@@ -1,5 +1,5 @@
 /*
- * qlora_b200 — C-ABI of the B200-native NF4 + double-quant Linear4bit hot path.
+ * qlora_b200 — C-ABI of the H100-native NF4 + double-quant Linear4bit hot path.
  *
  * This is the drop-in boundary: the entry points a bitsandbytes-style Python
  * host binds with ctypes for the path /root/reference/qlora.py reaches through
@@ -42,7 +42,7 @@ extern "C" {
 int qb200_version(void);
 /* Thread-local description of the last non-zero return code ("" if none). */
 const char* qb200_last_error(void);
-/* 1 if the library was compiled with the sm_100a fused tcgen05 path. */
+/* 1 if the library was compiled with the sm_90a fused wgmma path. */
 int qb200_has_fused_gemm(void);
 
 /* ---- arithmetic mode of the quantizers (K1, K2) -----------------------------------
@@ -86,7 +86,7 @@ int qb200_dequantize_nf4_nested(const uint8_t* packed, const uint8_t* absmax_u8,
                                 const float* absmax2, const float* offset, int64_t n, int blocksize, int blocksize2,
                                 void* out, int out_dtype, void* stream);
 
-/* ---- K5 (forward): fused dequant + tcgen05 GEMM -------------------------------------
+/* ---- K5 (forward): fused dequant + wgmma GEMM -------------------------------------
  * Replaces, for MatMul4Bit.forward [upstream autograd/_functions.py]:
  *   dequantize_4bit (K3, add, K4: bf16 W written to HBM)  +  torch.nn.functional.linear (cuBLAS).
  * Y[M,N] = X[M,K] . W[N,K]^T (+ bias[N]);  X,Y,bias bf16 row-major; W given by the nested
@@ -106,7 +106,7 @@ int qb200_nf4_linear_bwd_dx(const void* dY, const uint8_t* packed, const uint8_t
 
 /* ---- K5 + LoRA (SURVEY.md 8f-1): the caller's low-rank update folded into the same launch ----------------
  * Replaces peft lora.Linear4bit.forward's  `result = base(x); result += lora_B(lora_A(x)) * scaling`  (two extra GEMMs and
- * two elementwise passes over [M,N]) by one extra bf16 contraction step accumulated in the same TMEM accumulators:
+ * two elementwise passes over [M,N]) by one extra bf16 contraction step accumulated in the same register accumulators:
  *   forward : Y  = X . W^T (+bias) + U . V^T      U[M,R] = scaling * (X . A^T) (bf16),  V[N,R] = lora_B.weight
  *   backward: dX = dY . W          + U . Vt       U[M,R] = scaling * (dY . B)  (bf16),  Vt[R,K] = lora_A.weight
  * R: LoRA rank, a multiple of 8 in [8, 64] (columns/rows beyond R are zero-filled by TMA). */
@@ -134,7 +134,7 @@ int qb200_nf4_linear_ex(int is_bwd, const void* in, const uint8_t* packed, const
  * the three (two) separate MatMul4Bit calls on the SAME activation (q/k/v, gate/up) and, in backward, their three (two)
  * dX GEMMs plus autograd's accumulation of the input gradient:
  *   is_bwd = 0: out_p[M,N] = in_p . W_p^T (+bias_p) + U_p . V_p^T      for every problem p (in_p may be one tensor)
- *   is_bwd = 1: out_0[M,K] = sum_p ( in_p . W_p + U_p . V_p )           ONE output, accumulated in TMEM (out_p, p>0 ignored)
+ *   is_bwd = 1: out_0[M,K] = sum_p ( in_p . W_p + U_p . V_p )           ONE output, accumulated in registers (out_p, p>0 ignored)
  * Row pitches (elements; 0 = contiguous) let the outputs be column slices of one [M, nprob*N] buffer and U_p column
  * slices of one [M, nprob*R] projection.  out_dtype: QB200_DTYPE_BF16, or QB200_DTYPE_F32 = the bf16-rounded result
  * widened in the epilogue (Linear4bit.forward called with fp32 activations, qlora.py:396-405: no separate cast kernel).

@@ -1,9 +1,9 @@
-"""qlora_b200 — B200-native NF4 + double-quant Linear4bit hot path for QLoRA finetuning.
+"""qlora_b200 — H100-native NF4 + double-quant Linear4bit hot path for QLoRA finetuning.
 
 Drop-in for the slice of `bitsandbytes` that artidoro/qlora uses (qlora.py:15,249,318-326):
 `nn.Linear4bit`, `nn.Params4bit`, `matmul_4bit`, `functional.{quantize_4bit, dequantize_4bit,
-quantize_blockwise, dequantize_blockwise, QuantState}`.  The hot ops are hand-written sm_100a CUDA
-(TMA + in-register NF4 dequant + tcgen05 MMA) behind the C-ABI in include/qlora_b200.h.
+quantize_blockwise, dequantize_blockwise, QuantState}`.  The hot ops are hand-written sm_90a CUDA
+(TMA + in-register NF4 dequant + wgmma) behind the C-ABI in include/qlora_b200.h.
 `shims/bitsandbytes` re-exports this package under the import name `bitsandbytes`.
 """
 from . import functional, nn, optim  # noqa: F401

@@ -1,7 +1,7 @@
-"""In-tree build of libqlora_b200.so (hand-written sm_100a CUDA behind a C-ABI).
+"""In-tree build of libqlora_b200.so (hand-written sm_90a CUDA behind a C-ABI).
 
 `python -m qlora_b200._build` or `__graft_entry__.build()`.  nvcc cross-compiles
-for sm_100a without a GPU; the .so is git-ignored but travels to the GPU box.
+for sm_90a without a GPU; the .so is a build product and git-ignored.
 """
 from __future__ import annotations
 
@@ -13,9 +13,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libqlora_b200.so")
-SOURCES = ["qb200_api.cu", "nf4_quant.cu", "nf4_gemm_sm100.cu", "nf4_gemv.cu", "lora_proj.cu", "paged_optim.cu"]
+SOURCES = ["qb200_api.cu", "nf4_quant.cu", "nf4_gemm_sm90.cu", "nf4_gemv.cu", "lora_proj.cu", "paged_optim.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -53,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         subprocess.run(cmd, check=True)
         objs.append(obj)
     tmp = LIB_PATH + ".tmp"
-    subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp, *objs, "-cudart", "static"], check=True)
+    subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp, *objs, "-cudart", "static"], check=True)
     os.replace(tmp, LIB_PATH)
     return LIB_PATH
 

@@ -1,4 +1,4 @@
-"""`bitsandbytes.matmul_4bit` / `MatMul4Bit` on the fused B200 kernel.
+"""`bitsandbytes.matmul_4bit` / `MatMul4Bit` on the fused H100 kernel.
 
 Reference semantics being honoured (upstream bitsandbytes/autograd/_functions.py, reached from
 qlora.py:249 via `bnb.nn.Linear4bit.forward`; SURVEY.md 8a rows a8, a11):
@@ -7,8 +7,8 @@ qlora.py:249 via `bnb.nn.Linear4bit.forward`; SURVEY.md 8a rows a8, a11):
     backward: grad_A = grad_out @ dequantize_4bit(B, state).to(grad_out.dtype).t()   (B is weight.t())
               grad_B = None (frozen base weight: no dW GEMM), grad_bias = grad_out.sum(0)
 
-Here forward and dX run as ONE hand-written sm_100a kernel each (NF4 nibbles -> bf16 tiles in
-shared memory -> tcgen05.mma), so the dequantized W never reaches HBM.  Inputs the fused kernel
+Here forward and dX run as ONE hand-written sm_90a kernel each (NF4 nibbles -> bf16 tiles in
+shared memory -> wgmma), so the dequantized W never reaches HBM.  Inputs the fused kernel
 does not cover (fp16/fp32 compute dtype, K % 64 != 0, ...) take the unfused *GPU* path
 (our dequant kernel + cuBLAS), which is also the "bnb-equivalent" baseline timed in bench.py.
 """

@@ -8,7 +8,7 @@
 #include <stdlib.h>
 
 #include "qb200_internal.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace qb200 {
 

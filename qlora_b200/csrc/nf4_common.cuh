@@ -1,4 +1,4 @@
-// Shared device helpers for the NF4 + double-quant kernels (sm_100a only).
+// Shared device helpers for the NF4 + double-quant kernels (sm_90a).
 //
 // Numeric contract (SURVEY.md Appendix A; bitsandbytes csrc/kernels.cu
 // dQuantizeNF4 / dDequantizeNF4 / dQuantize<0> [upstream, un-vendored]):

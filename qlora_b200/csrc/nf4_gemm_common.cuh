@@ -1,6 +1,6 @@
-// Shared pieces of the fused NF4 dequant + tcgen05 GEMM kernels (sm_100a): launch parameters, the register-resident
+// Shared pieces of the fused NF4 dequant + wgmma GEMM kernel (sm_90a): launch parameters, the register-resident
 // product-table dequant (16 x bf16_rne(LUT[j]*absmax) per NF4 block, nibbles resolved with PRMT byte permutes), the
-// nested-absmax prefetch helper and the UMMA shared-memory descriptors.
+// nested-absmax prefetch helper and the wgmma shared-memory descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -10,17 +10,17 @@
 #include "nf4_common.cuh"
 #include "nf4_table.cuh"
 #include "qb200_internal.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace qb200 {
 namespace gemm {
 
-constexpr int kBlockF = 128;   // features per CTA (UMMA M per CTA)
+constexpr int kBlockF = 128;   // features per work unit (two wgmma M=64 halves)
 constexpr int kBlockC = 64;    // contraction per step (one NF4 block; 128 B of bf16 = one swizzle row)
-constexpr int kUmmaK = 16;
-constexpr int kATileBytes = kBlockF * kBlockC * 2;    // 16 KB: one dequantized UMMA A-operand tile
+constexpr int kMmaK = 16;
+constexpr int kATileBytes = kBlockF * kBlockC * 2;    // 16 KB: one dequantized wgmma A-operand tile
 constexpr int kWTileBytes = kBlockF * kBlockC / 2;    // 4 KB: the packed nibbles of that tile
-constexpr int kAuxBytes = 1024 + 3 * 1024;            // barriers + tmem slot (1 KB), one code256 copy per problem of a group
+constexpr int kAuxBytes = 1024 + 3 * 1024;            // barriers (1 KB), one code256 copy per problem of a group
 
 constexpr int kMaxProb = 3;    // problems per grouped launch (q/k/v, gate/up)
 
@@ -47,6 +47,7 @@ struct Params {
   int N;                     // rows of W
   int lora_r;                // > 0: one extra bf16 contraction step per problem  Out += U_p[T,r] . V_p^T
   int out_f32;               // 1: the drain writes fp32 (Linear4bit called with fp32 activations: no separate cast pass)
+  float* ws;                 // split-K: fp32 partial sums [ksplit, T, F] (null otherwise)
   int debug;                 // ablation flags for performance triage (QB200_DEBUG_FLAGS; 0 in production):
                              //   1 = skip dequant math+stores, 2 = skip MMA issue, 4 = skip epilogue stores
 };
@@ -75,16 +76,17 @@ struct AbsmaxFetch {
   }
 };
 
+// wgmma shared-memory matrix descriptors (sm_90): start >> 4 at [0,14), LBO >> 4 at [16,30), SBO >> 4 at [32,46),
+// base offset 0 (tiles are 1024-byte aligned), layout type at [62,64): 1 = SWIZZLE_128B.
 __device__ __forceinline__ uint64_t make_desc_kmajor_sw128(uint32_t smem_addr) {
   // K-major, SWIZZLE_128B: rows of 128 B, 8-row groups 1024 B apart (SBO); LBO unused (=1).
-  return uint64_t((smem_addr >> 4) & 0x3FFFu) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) |
-         (uint64_t(2) << 61);
+  return uint64_t((smem_addr >> 4) & 0x3FFFu) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
 __device__ __forceinline__ uint64_t make_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   // MN-major, SWIZZLE_128B: atoms of 64 (MN) x 8 (K) elements = 1024 B; LBO = stride between
   // 64-element groups along MN, SBO = stride between 8-row groups along K.
   return uint64_t((smem_addr >> 4) & 0x3FFFu) | (uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         (uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32) | (uint64_t(1) << 46) | (uint64_t(2) << 61);
+         (uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32) | (uint64_t(1) << 62);
 }
 
 }  // namespace gemm

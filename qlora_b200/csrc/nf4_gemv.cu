@@ -3,7 +3,7 @@
 //
 // Replaces the reference's bs-1 generation path (SURVEY.md 2.4 K6 `kgemm_4bit_inference_naive`, reached from
 // examples/guanaco_generate.py:63-78 and qlora.py:817-834 through bnb.matmul_4bit when A.numel() == A.shape[-1];
-// README.md:135 calls 4-bit inference slow) and the few-token forward calls below the tcgen05 tile sizes.
+// README.md:135 calls 4-bit inference slow) and the few-token forward calls below the wgmma tile sizes.
 // The packed weight (N*K/2 B) + u8 absmax (N*K/64 B) are streamed exactly once; W is never materialised.
 //
 // Warp-level tensor-core path (mma.sync m16n8k16 bf16, fp32 accumulate) — the one place this library uses mma.sync:
@@ -25,7 +25,7 @@
 #include "nf4_common.cuh"
 #include "nf4_table.cuh"
 #include "qb200_internal.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace qb200 {
 namespace skinny {
@@ -68,7 +68,7 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], uint32_t a0, uint3
 }
 
 // LoRA term of one output value: sum_j U[m, j] * V[row, j] over the rank (bf16 operands, fp32 sum) — the extra contraction
-// step the pair kernel runs on the tensor core, here 8..64 multiply-adds in the epilogue.  U = scaling * x . A^T [M, r] comes
+// step the wgmma kernel runs on the tensor core, here 8..64 multiply-adds in the epilogue.  U = scaling * x . A^T [M, r] comes
 // from the caller (one small GEMM), V = lora_B.weight [N, r]; rows are 16-byte aligned (r % 8 == 0).
 __device__ __forceinline__ float lora_dot(const __nv_bfloat16* __restrict__ u, const __nv_bfloat16* __restrict__ v, int r) {
   // all (at most 8 + 8) 16-byte loads are issued before the first multiply: one memory round trip, not r / 8 of them
@@ -266,7 +266,7 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
   }
 }
 
-// Launch with programmatic stream serialization (QB200_PDL=0 disables it, as for the pair kernel).
+// Launch with programmatic stream serialization (QB200_PDL=0 disables it, as for the wgmma kernel).
 template <typename Kern, typename... Args>
 static int launch_pdl(Kern kern, unsigned grid, unsigned block, int smem, cudaStream_t stream, const char* what, Args... args) {
   static const bool pdl = [] {

@@ -1,4 +1,4 @@
-// NF4 / 8-bit blockwise quantize + dequantize kernels for sm_100a (K1-K4 of SURVEY.md 2.4).
+// NF4 / 8-bit blockwise quantize + dequantize kernels for sm_90a (K1-K4 of SURVEY.md 2.4).
 //
 // These are HBM-bound streaming kernels: 128-bit coalesced loads/stores, one 32-bit
 // packed word (8 NF4 codes) per thread, no shared-memory staging needed (no reuse).
@@ -499,8 +499,8 @@ __global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __
     Nf4Table tab;
     build_table<T16>(am, tab);
     uint8_t* dst = out + (uint64_t(i) << 6);
-    ptx::st_global_256(dst, dequant_word(w.x, tab), dequant_word(w.y, tab));
-    ptx::st_global_256(dst + 32, dequant_word(w.z, tab), dequant_word(w.w, tab));
+    ptx::st_global_32B(dst, dequant_word(w.x, tab), dequant_word(w.y, tab));
+    ptx::st_global_32B(dst + 32, dequant_word(w.z, tab), dequant_word(w.w, tab));
   }
 }
 
@@ -533,7 +533,8 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
           !dequant_lut_path()) {
         const uint32_t nvec = uint32_t(n / 32);
         int64_t tb = (int64_t(nvec) + threads - 1) / threads;
-        if (tb > 148LL * 4) tb = 148LL * 4;
+        const int64_t tb_max = int64_t(device_sm_count()) * 4;   // persistent grid: 4 CTAs per SM
+        if (tb > tb_max) tb = tb_max;
         if (absmax_u8 != nullptr)
           dequantize_nf4_tab_kernel<T, true><<<(unsigned)tb, threads, 0, stream>>>(
               reinterpret_cast<const uint4*>(packed), nullptr, absmax_u8, code256, absmax2, offset, nvec, bs_shift - 2, bs2_shift,
@@ -544,7 +545,8 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
               reinterpret_cast<uint8_t*>(out));
         return check_launch("dequantize_nf4");
       }
-      int64_t fb = blocks > 148LL * 16 ? 148LL * 16 : blocks;
+      const int64_t fb_max = int64_t(device_sm_count()) * 16;
+      const int64_t fb = blocks > fb_max ? fb_max : blocks;
       if (absmax_u8 != nullptr)
         dequantize_nf4_fast_kernel<T, true><<<(unsigned)fb, threads, 0, stream>>>(
             reinterpret_cast<const uint32_t*>(packed), nullptr, absmax_u8, code256, absmax2, offset, uint32_t(nwords), bs_shift,
@@ -556,7 +558,7 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
       return check_launch("dequantize_nf4");
     }
   }
-  const int64_t max_blocks = 148LL * 8 * 8;  // grid-stride beyond a few waves of 8 resident CTAs/SM
+  const int64_t max_blocks = int64_t(device_sm_count()) * 8 * 8;  // grid-stride beyond a few waves of 8 resident CTAs/SM
   if (blocks > max_blocks) blocks = max_blocks;
   if (absmax_u8 != nullptr) {
     dequantize_nf4_kernel<T, true><<<(unsigned)blocks, threads, 0, stream>>>(packed, nullptr, absmax_u8, code256, absmax2,
@@ -601,7 +603,7 @@ extern "C" int qb200_quantize_blockwise_8bit(const float* code256, const float* 
   if (n == 0) return 0;
   const int64_t nblocks = (n + blocksize - 1) / blocksize;
   int64_t blocks = (nblocks + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > int64_t(device_sm_count()) * 8) blocks = int64_t(device_sm_count()) * 8;
   if (quant_math())
     quantize_8bit_kernel<true><<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(code256, A, n, blocksize, out, absmax);
   else
@@ -615,7 +617,7 @@ extern "C" int qb200_dequantize_blockwise_8bit(const float* code256, const uint8
   if (blocksize <= 0) return set_error(QB200_EINVAL, "dequantize_8bit: blocksize must be positive");
   if (n == 0) return 0;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > int64_t(device_sm_count()) * 8) blocks = int64_t(device_sm_count()) * 8;
   dequantize_8bit_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(code256, A, absmax, n, blocksize, out);
   return check_launch("dequantize_blockwise_8bit");
 }

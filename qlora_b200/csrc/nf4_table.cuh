@@ -1,6 +1,6 @@
 // Register-resident product table of one NF4 block: the 16 values  T16_rne(LUT[j] * absmax)  a block can take, kept as
 // low-byte / high-byte planes so that PRMT byte permutes resolve 4 nibbles at a time (2 PRMT per weight, nothing else per
-// weight: no shared-memory look-up, no multiply, no convert).  Shared by the fused GEMM (nf4_gemm_pair.cuh), the skinny
+// weight: no shared-memory look-up, no multiply, no convert).  Shared by the fused GEMM (nf4_gemm_wgmma.cuh), the skinny
 // forward (nf4_gemv.cu) and the standalone dequantize kernel (nf4_quant.cu): all three emit bit-identical weights.
 #pragma once
 #include <cuda_bf16.h>
@@ -9,7 +9,7 @@
 #include <type_traits>
 
 #include "nf4_common.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace qb200 {
 

@@ -71,7 +71,7 @@ static int launch_adamw_dev(void* p, const void* g, float* m, float* v, int64_t 
                             float weight_decay, const float* step_dev, const float* gnorm_scale_dev, cudaStream_t stream) {
   const float decay = weight_decay > 0.0f ? 1.0f - lr * weight_decay : 1.0f;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > int64_t(device_sm_count()) * 16) blocks = int64_t(device_sm_count()) * 16;
   adamw32bit_dev_kernel<T><<<unsigned(blocks), 256, 0, stream>>>(static_cast<T*>(p), static_cast<const T*>(g), m, v, n, lr, beta1, beta2,
                                                                 eps, decay, step_dev, gnorm_scale_dev);
   return check_launch("adamw32bit_step_dev");
@@ -85,7 +85,7 @@ static int launch_adamw(void* p, const void* g, float* m, float* v, int64_t n, f
   const float step_size = -lr * c2 / c1;
   const float decay = weight_decay > 0.0f ? 1.0f - lr * weight_decay : 1.0f;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > int64_t(device_sm_count()) * 16) blocks = int64_t(device_sm_count()) * 16;
   adamw32bit_kernel<T><<<unsigned(blocks), 256, 0, stream>>>(static_cast<T*>(p), static_cast<const T*>(g), m, v, n, beta1, beta2,
                                                             eps * c2, step_size, decay, gnorm_scale);
   return check_launch("adamw32bit_step");

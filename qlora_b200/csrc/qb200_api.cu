@@ -21,6 +21,18 @@ int check_launch(const char* what) {
   snprintf(t_last_error, sizeof(t_last_error), "%s: %s (%s)", what, cudaGetErrorName(err), cudaGetErrorString(err));
   return int(err);
 }
+
+int device_sm_count() {
+  constexpr int kMaxDevices = 16;
+  static int sms[kMaxDevices] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
+  if (sms[dev] == 0) {
+    int n = 0;
+    sms[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
+  }
+  return sms[dev];
+}
 }  // namespace qb200
 
 extern "C" int qb200_version(void) { return 100; /* 0.1.0 */ }

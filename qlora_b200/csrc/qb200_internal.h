@@ -10,6 +10,8 @@ namespace qb200 {
 int set_error(int code, const char* msg);
 // cudaPeekAtLastError() after a launch -> 0 or the cudaError_t (message recorded).
 int check_launch(const char* what);
+// Streaming multiprocessors of the calling thread's current device (cached per device); grid sizes are multiples of it.
+int device_sm_count();
 // Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16, with an optional LoRA term U[M,R] . V[N,R]^T;
 // ld_* are row pitches in elements (0 = dense).
 int launch_nf4_skinny(const void* x, int64_t ld_x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,

@@ -1,4 +1,4 @@
-"""`bitsandbytes.functional` surface for the NF4 + double-quant path, on B200-native kernels.
+"""`bitsandbytes.functional` surface for the NF4 + double-quant path, on H100-native kernels.
 
 Mirrors (names, argument meaning, return shapes, error behaviour) the upstream functions the
 reference reaches through `qlora.py:15,249,318-326` (SURVEY.md 8b):
@@ -8,7 +8,7 @@ reference reaches through `qlora.py:15,249,318-326` (SURVEY.md 8b):
     QuantState (+ as_dict/from_dict/to, list-style indexing)
     create_dynamic_map, create_normal_map, get_4bit_type
 
-All device work goes through the C-ABI in include/qlora_b200.h (hand-written sm_100a CUDA).
+All device work goes through the C-ABI in include/qlora_b200.h (hand-written sm_90a CUDA).
 CUDA tensors only: there is no CPU implementation in this package (the CPU restatement lives
 in oracle/ and is test infrastructure).
 """
@@ -242,7 +242,7 @@ def _require_cuda(*tensors: Optional[Tensor]) -> torch.device:
             continue
         if not t.is_cuda:
             raise RuntimeError(
-                "qlora_b200 ops run on CUDA tensors only (B200-native kernels, no CPU fallback); "
+                "qlora_b200 ops run on CUDA tensors only (H100-native kernels, no CPU fallback); "
                 f"got a tensor on {t.device}"
             )
         if dev is None:
@@ -423,7 +423,7 @@ def dequantize_nf4(A, quant_state=None, absmax=None, out=None, blocksize=64):
 # --------------------------------------------------------------------------------------
 
 def fused_supported(quant_state: QuantState, compute_dtype: torch.dtype) -> bool:
-    """Shapes/dtypes the fused tcgen05 kernel handles; everything else takes the unfused GPU path."""
+    """Shapes/dtypes the fused wgmma kernel handles; everything else takes the unfused GPU path."""
     if compute_dtype != torch.bfloat16 or quant_state.quant_type != "nf4" or quant_state.blocksize != 64:
         return False
     if quant_state.shape is None or len(quant_state.shape) != 2 or quant_state.dtype != torch.bfloat16:

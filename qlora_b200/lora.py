@@ -6,7 +6,7 @@ peft's `lora.Linear4bit.forward` (reached from qlora.py:386-394 `get_peft_model`
     result = result + lora_B(lora_A(dropout(x))) * scaling
 
 i.e. two more GEMMs plus scale/add passes over [M, N] (and their mirror images in backward).  Here the low-rank
-update is ONE extra bf16 contraction step of the fused kernel, accumulated in the same TMEM accumulators:
+update is ONE extra bf16 contraction step of the fused kernel, accumulated in the same register accumulators:
 
     forward : Y  = X . W^T + U . B^T         U = scaling * (drop(X) . A^T)   [M, r]
     backward: dX = dY . W  + G . A           G = scaling * (dY . B)          [M, r]
@@ -22,7 +22,7 @@ fused dX launch carries the base term only.
 
 Linears that share their input and shape (q/k/v, gate/up) run as ONE grouped launch per direction
 (`lora_linear4bit_group`): the three (two) forward GEMMs side by side, the backward as one long contraction
-dX = sum_p (dY_p . W_p + G_p . A_p) accumulated in TMEM — no separate accumulation of the input gradient — and the
+dX = sum_p (dY_p . W_p + G_p . A_p) accumulated in the same accumulators — no separate accumulation of the input gradient — and the
 `x . A_p^T` projections batched into one GEMM.
 
 fp32 activations (the reference casts its norms to fp32, qlora.py:400-401, so `Linear4bit.forward` sees fp32 in and

@@ -2,7 +2,7 @@
 
 Put `<repo>/shims` on PYTHONPATH (see INTEGRATION.md) and the reference's three touch-points
 (qlora.py:15 import, qlora.py:249 `bnb.nn.Linear4bit`/`bnb.nn.Linear8bitLt`, qlora.py:318-326
-BitsAndBytesConfig -> HF -> `bnb.nn.Linear4bit(...)`, `bnb.nn.Params4bit(...)`) bind to the B200 path.
+BitsAndBytesConfig -> HF -> `bnb.nn.Linear4bit(...)`, `bnb.nn.Params4bit(...)`) bind to the H100 path.
 """
 import os as _os
 import sys as _sys

@@ -54,24 +54,24 @@ def test_argument_errors_do_not_need_a_gpu():
     assert lib.qb200_nf4_linear_fwd(p, p, None, None, None, None, None, None, p, 8, 128, 128, None) == -1  # no absmax
 
 
-def test_sass_is_blackwell_native():
-    """The shipped .so must contain tcgen05 / TMA / TMEM SASS (UTCHMMA, UTMALDG, LDTM)."""
+def test_sass_is_hopper_native():
+    """The shipped .so must contain sm_90a warpgroup-MMA and TMA SASS (HGMMA, UTMALDG)."""
     from qlora_b200 import _lib
 
     cuobjdump = "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "UTMASTG", "LDTM"):
+    for mnemonic in ("HGMMA", "UTMALDG"):
         assert mnemonic in sass, mnemonic
     # warp-level mma.sync (HMMA) is allowed in exactly one place: the <= 32-token skinny forward kernel, which is bound by the
     # NF4 look-up on the ALU pipe and feeds the look-up registers straight into the MMA (DESIGN.md); every GEMM-sized
-    # launch is tcgen05 (UTCHMMA)
+    # launch is wgmma (HGMMA)
     fn = None
     for line in sass.splitlines():
         if "Function :" in line:
             fn = line
-        elif "HMMA." in line and "UTCHMMA" not in line:
+        elif "HMMA." in line:
             assert fn is not None and "nf4_skinny_kernel" in fn, fn
 
 

@@ -1,8 +1,8 @@
-"""GPU parity: fused NF4 dequant + tcgen05 GEMM (forward and dX) vs the oracle.
+"""GPU parity: fused NF4 dequant + wgmma GEMM (forward and dX) vs the oracle.
 
 Tolerance (north_star: "within 1e-3 relative bf16"): ||Y - Y_ref||_F / ||Y_ref||_F <= 1e-3 with both sides
 bf16-rounded, AND every element within one bf16 ulp (2^-8 of the largest magnitude) of the reference —
-summation order differs between tcgen05, cuBLAS and the CPU, so an fp32 accumulator can round to the
+summation order differs between wgmma, cuBLAS and the CPU, so an fp32 accumulator can round to the
 adjacent bf16 value (a max-norm bound below one ulp is unattainable for ANY bf16 GEMM, cuBLAS included).
 The dequantized weights feeding the tensor core ARE bit-exact (identity-input test below)."""
 import numpy as np
@@ -208,7 +208,7 @@ def test_fused_lora_autograd_matches_unfused(q):
 @pytest.mark.parametrize("m", [1, 16, 48, 64, 80, 300, 512, 1024])
 def test_small_m_split_k(q, c_oracle, m):
     """Small token counts: the split-K schedule (fp32 partials in a lent workspace + reduce) for the smallest, the range
-    schedule with few-token units (UMMA N = 16..) above — forward with bias, dX, and the fused-LoRA forms, all against
+    schedule with few-token units (wgmma N = 16..) above — forward with bias, dX, and the fused-LoRA forms, all against
     the oracle.  The library decides (qb200_nf4_linear_workspace_size > 0 <=> split-K)."""
     F = q.functional
     from qlora_b200 import _lib
@@ -268,7 +268,7 @@ def test_gemv_small_batch(q, c_oracle, m, n, k, nested):
 @pytest.mark.parametrize("n,k", [(4096, 4096), (200, 192), (8, 64), (24, 320), (4096, 11008)])
 def test_skinny_forward_up_to_32_tokens(q, c_oracle, m, n, k, nested):
     """Forward calls with 1..16 tokens and no LoRA operands run the warp-level skinny kernel (nf4_gemv.cu: mma.sync with the
-    PRMT look-up output as B fragment, x staged through shared memory); 17..32 tokens cross over to the split-K pair kernel.
+    PRMT look-up output as B fragment, x staged through shared memory); 17..32 tokens cross over to the split-K wgmma kernel.
     Shapes include K/64 not a multiple of 4 (partial block groups, zero-filled slabs) and N = 8."""
     F = q.functional
     w = make_weight(n, k, seed=3 * n + k)
@@ -358,7 +358,7 @@ def test_grouped_launch_small_shapes_vs_oracle(q, c_oracle, m, n, k, r, nprob, n
     """`qb200_nf4_linear_group`: ragged token counts (not multiples of 16), feature counts that are not multiples of 256,
     one- and two-step contractions with a LoRA step after every segment, strided U, outputs written as column slices of ONE
     buffer — forward side by side and the backward contraction-sum, against the oracle.  With 16 tokens or fewer the forward is
-    one skinny launch per problem (pitched outputs and U included), the backward still the pair kernel."""
+    one skinny launch per problem (pitched outputs and U included), the backward still the wgmma kernel."""
     F = q.functional
     packs, states, w_refs = [], [], []
     for i in range(nprob):
@@ -397,7 +397,7 @@ def test_grouped_launch_small_shapes_vs_oracle(q, c_oracle, m, n, k, r, nprob, n
 @pytest.mark.parametrize("m,n,k", [(2048, 512, 256), (1500, 768, 512), (1040, 256, 128)])
 def test_range_schedule_units_bit_equal_across_token_counts(q, m, n, k):
     """The range schedule cuts the token axis wherever the cost model says; an output row must not depend on which unit
-    (UMMA N = 16..256, one or two blocks) computed it: rows of a short call equal the same rows of a long call bit for bit.
+    (wgmma N = 16..128) computed it: rows of a short call equal the same rows of a long call bit for bit.
     (Token counts the library serves with the split-K schedule sum fp32 partials in another order: one bf16 ulp allowed.)"""
     F = q.functional
     from qlora_b200 import _lib
@@ -534,7 +534,7 @@ def test_skinny_forward_with_lora_operands(q, c_oracle, m, r, n, k, nested):
     v = make_weight(n, r, seed=22 + r, scale=0.05)
     bias = make_weight(1, n, seed=9, scale=0.5).view(-1)
     ws = F._lib.load().qb200_nf4_linear_workspace_size(m, n, k, 0)
-    assert ws == 0                                        # no split-K workspace: not the pair kernel
+    assert ws == 0                                        # no split-K workspace: not the wgmma kernel
     for b in (None, bias):
         y = F.nf4_linear_fwd_lora(x, packed, qs, u, v, b)
         y_ref = bf16_to_f32_np(x) @ w_ref.T + bf16_to_f32_np(u.contiguous()) @ bf16_to_f32_np(v).T

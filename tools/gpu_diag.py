@@ -123,7 +123,7 @@ def run_step(name):
         _check_linear(name, 2048, 512, 4096, True, do_bwd=False)
     elif name == "bwd_mid":
         _check_linear(name, 2048, 512, 4096, True, do_fwd=False)
-    elif name == "tail_split":  # 11008-wide: 172 tiles -> 148 whole + 24 split into 48 halves on 74 SM pairs
+    elif name == "tail_split":  # 11008-wide: 86 feature blocks, ranges that end inside a block's token strip
         _check_linear(name, 2048, 11008, 512, True)
         _check_linear(name + "_1000tok", 1000, 640, 512, True)
     elif name == "perf":

@@ -1,5 +1,5 @@
 // Issue rates of the integer instructions the NF4 look-up is made of, per SM and clock, on the GPU this runs on.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench/alu_rates tools/microbench/alu_rates.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench/alu_rates tools/microbench/alu_rates.cu
 // Each kernel runs kIters x 32 independent instructions of one kind per thread (8 accumulators x 4), with enough warps
 // (1..8 per SM sub-partition) to saturate the pipe; rate = warp instructions x 32 lanes / (SM cycles).
 #include <cstdint>

@@ -3,7 +3,7 @@
 //   method 0: per-block product table (16 x bf16(LUT[j] * absmax) as byte planes), nibbles resolved with PRMT   (production)
 //   method 1: constant fp32 LUT in shared memory: nibble -> byte offset -> LDS -> FMUL by absmax -> cvt.rn.bf16x2
 //   method 2: half of the words by method 0, half by method 1
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I qlora_b200/csrc -o tools/microbench/lookup_rates tools/microbench/lookup_rates.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I qlora_b200/csrc -o tools/microbench/lookup_rates tools/microbench/lookup_rates.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

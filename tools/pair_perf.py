@@ -1,4 +1,4 @@
-"""Per-launch timings of the pair kernel at the model shapes bench.py runs (CUDA events, L2 flushed between iterations,
+"""Per-launch timings of the fused wgmma kernel at the model shapes bench.py runs (CUDA events, L2 flushed between iterations,
 median of N): single, fused-LoRA and grouped launches next to cuBLAS on pre-dequantized bf16 weights and to the
 bnb-equivalent dequantize + cuBLAS sequence.  One JSON line per case on stdout.
 

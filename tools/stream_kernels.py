@@ -43,7 +43,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("hbm_gbs", 6650.0)
+    peak = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet (HBM3)
     only_gemv = bool(int(os.environ.get("QB200_ONLY_GEMV", "0")))
     for n, k in ((4096, 4096), (11008, 4096), (4096, 11008)):
         nel = n * k

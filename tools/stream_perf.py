@@ -1,7 +1,7 @@
 """Timing of the HBM-streaming kernels of the library (SURVEY.md 8d: K1 quantize, K4 dequantize, the few-token skinny
 forward) against the measured HBM copy bandwidth.
 
-Every case is a CUDA graph of `reps` launches that rotate over enough distinct weight copies to exceed the 126 MB L2
+Every case is a CUDA graph of `reps` launches that rotate over enough distinct weight copies to exceed the 50 MB L2
 (no flush kernels inside the timed region; every launch reads its operands from HBM), timed with CUDA events; the
 per-launch figure is graph time / reps, so it includes the back-to-back launch gap a decode loop would see.
 
@@ -37,8 +37,8 @@ from gpu_helpers import make_act, make_weight  # noqa: E402
 try:
     PEAK = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
-    PEAK = 6564.8
-L2_BYTES = 126 << 20
+    PEAK = 3350.0   # H100 SXM data sheet (HBM3)
+L2_BYTES = 50 << 20   # H100 L2
 SHAPES = [(4096, 4096), (11008, 4096), (4096, 11008)]
 WHAT = set(args.what.split(","))
 lines = []
