@@ -85,7 +85,7 @@ class LoRALinear4bit(nn.Module):
 
     _next_salt = [1]
 
-    def __init__(self, base, r: int, alpha: int, dropout: float, device=None, seed_tensor=None, generator=None):
+    def __init__(self, base, r: int, alpha: int, dropout: float, device=None, seed_tensor=None, generator=None, use_dora=False):
         super().__init__()
         self.base_layer = base
         self.lora_A = nn.Linear(base.in_features, r, bias=False, dtype=torch.bfloat16, device=device)
@@ -99,6 +99,10 @@ class LoRALinear4bit(nn.Module):
         self.salt = LoRALinear4bit._next_salt[0]     # call-site id of the seeded dropout
         LoRALinear4bit._next_salt[0] += 1
         self._seed = [seed_tensor]                   # in a list: not a registered buffer, shared by every adapter
+        self.use_dora = use_dora
+        if use_dora:   # peft's lora_magnitude_vector: ||W_f|| of the frozen base (B = 0), in the adapters' dtype
+            self.magnitude = nn.Parameter(bnb.functional.weight_row_norm2(base.weight.data, base.weight.quant_state).sqrt()
+                                          .to(torch.bfloat16))
 
     def lora_input(self, x):
         """The LoRA branch's input `dropout(x)`, or None when it is x itself (p = 0 / eval)."""
@@ -113,6 +117,12 @@ class LoRALinear4bit(nn.Module):
         return self.fused and isinstance(self.base_layer, bnb.nn.Linear4bit)
 
     def forward(self, x):
+        if self.use_dora:
+            if self.is_fusable():   # the magnitude rides in the NF4 kernels as a per-row weight scale
+                return bnb.dora_linear4bit(x, self.base_layer, self.lora_A.weight, self.lora_B.weight, self.magnitude, self.scaling,
+                                           self.lora_input(x))
+            return bnb.dora_linear4bit_peft(x, self.base_layer, self.lora_A.weight, self.lora_B.weight, self.magnitude, self.scaling,
+                                            self.lora_input(x))
         if self.is_fusable():
             # SURVEY.md 8f-1: the low-rank update rides in the NF4 GEMM as one extra bf16 contraction step
             return bnb.lora_linear4bit(x, self.base_layer, self.lora_A.weight, self.lora_B.weight, self.scaling, self.lora_input(x))
@@ -129,8 +139,13 @@ class LoRALinear4bit(nn.Module):
 
 def lora_group(mods, x):
     """q/k/v (gate/up): LoRA-wrapped Linear4bit of one shape on one input -> ONE grouped launch per direction."""
-    if GROUP_LINEARS and all(isinstance(m, LoRALinear4bit) and m.is_fusable() for m in mods) and len({m.scaling for m in mods}) == 1:
+    if (GROUP_LINEARS and all(isinstance(m, LoRALinear4bit) and m.is_fusable() for m in mods) and len({m.scaling for m in mods}) == 1
+            and len({m.use_dora for m in mods}) == 1):
         xls = [m.lora_input(x) for m in mods]
+        if mods[0].use_dora:
+            return bnb.dora_linear4bit_group(x, [m.base_layer for m in mods], [m.lora_A.weight for m in mods],
+                                             [m.lora_B.weight for m in mods], [m.magnitude for m in mods], mods[0].scaling,
+                                             None if all(t is None for t in xls) else xls)
         return bnb.lora_linear4bit_group(x, [m.base_layer for m in mods], [m.lora_A.weight for m in mods],
                                          [m.lora_B.weight for m in mods], mods[0].scaling,
                                          None if all(t is None for t in xls) else xls)
@@ -228,7 +243,7 @@ def quantize_with_hf(model: nn.Module, double_quant: bool = True):
 
 class LlamaQLoRA(nn.Module):
     def __init__(self, shape: LlamaShape, device, lora_r=64, lora_alpha=16, lora_dropout=0.0, seed=0,
-                 double_quant=True, grad_checkpointing=True, quantized=True, norm_out_fp32=False):
+                 double_quant=True, grad_checkpointing=True, quantized=True, norm_out_fp32=False, use_dora=False):
         super().__init__()
         self.shape = shape
         self.grad_checkpointing = grad_checkpointing
@@ -274,7 +289,7 @@ class LlamaQLoRA(nn.Module):
             for layer in self.layers:
                 for name in targets:
                     setattr(layer, name, LoRALinear4bit(getattr(layer, name), lora_r, lora_alpha, lora_dropout, device, self.dropout_seed,
-                                                          generator=gen))
+                                                          generator=gen, use_dora=use_dora))
                 # adapters that are used together live side by side: lora_A of q/k/v (gate/up) are row blocks of ONE buffer, so
                 # the grouped launch's batched projection x . [A_q; A_k; A_v]^T needs no concatenation (same values, same init)
                 for grp in (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj")):

@@ -158,6 +158,17 @@ typedef struct qb200_nf4_problem {
 int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M, int64_t N, int64_t K,
                            int out_dtype, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- grouped form with a per-row weight scale (DoRA's magnitude over the NF4 base) ------------------------------------
+ * Same as qb200_nf4_linear_group, with W_p replaced by diag(s_p) . W_p:  row_scales[p] is a DEVICE fp32 array of N values
+ * (4-byte aligned) or NULL (problem p unscaled).  The scale multiplies the absmax of every NF4 block of row n, so
+ *   is_bwd = 0: out_p = in_p . (diag(s_p) W_p)^T (+bias_p) + U_p . V_p^T      (s_p scales output feature n)
+ *   is_bwd = 1: out_0 = sum_p ( in_p . diag(s_p) W_p + U_p . V_p )             (s_p scales contraction index n)
+ * The LoRA term and the bias are not scaled.  row_scales itself is a HOST array of nprob pointers and must not be NULL.
+ * The scales may be written by the preceding kernel on the stream; a scaled launch reads them only after that kernel is done. */
+int qb200_nf4_linear_group_scaled(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales, int64_t R,
+                                  int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
+                                  void* stream);
+
 /* U[M,R] = scale * X[M,K] . A[R,K]^T for 1..16 tokens (bf16 in / out, fp32 sum, one rounding): the lora_A projection that
  * feeds qb200_nf4_linear_group's U operand during generation with an unmerged adapter — peft `lora.Linear.forward`'s
  * `lora_A(dropout(x))` (qlora.py:817-834 through PeftModel); replaces a split-K cuBLAS GEMM + reduce per projection.

@@ -33,6 +33,8 @@ struct Prob {
   const float* offset;
   const float* absmax_f32;   // non-nested state (or null)
   const __nv_bfloat16* bias; // [F] or null (forward only)
+  const float* row_scale;    // [N] or null: the absmax of every NF4 block of row n of W is multiplied by row_scale[n]
+                             // (forward: Out = In . (diag(s) W)^T; dX: Out = In . diag(s) W).  Written by earlier kernels.
   void* out;                 // [T, F] bf16 (or fp32 when Params::out_f32), row pitch ld_out elements
   int64_t ld_out;
 };

@@ -269,6 +269,7 @@ struct GroupArgs {
   int out_f32;
   void* workspace;
   int64_t workspace_bytes;
+  const float* const* row_scales;   // [nprob] or null; an entry may be null (that problem is unscaled)
 };
 
 template <bool kTrans>
@@ -314,6 +315,7 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     d.offset = q.offset;
     d.absmax_f32 = q.absmax_u8 ? nullptr : q.absmax_f32;
     d.bias = static_cast<const __nv_bfloat16*>(q.bias);
+    d.row_scale = g.row_scales ? g.row_scales[i] : nullptr;
     d.out = p.group_sum ? g.pr[0].out : q.out;
     d.ld_out = (p.group_sum ? g.pr[0].ld_out : q.ld_out) > 0 ? (p.group_sum ? g.pr[0].ld_out : q.ld_out) : F;
   }
@@ -430,9 +432,9 @@ using namespace qb200;
 
 extern "C" int qb200_has_fused_gemm(void) { return 1; }
 
-// ---- general entry point: 1..3 problems of one shape in ONE launch ----------------------------------------------------
-extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M, int64_t N,
-                                      int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
+// ---- general entry point: 1..3 problems of one shape in ONE launch, each with an optional row scale ------------------
+static int linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales, int64_t R, int64_t M,
+                        int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
   if (out_dtype != QB200_DTYPE_BF16 && out_dtype != QB200_DTYPE_F32)
     return set_error(QB200_EINVAL, "nf4_linear_group: out_dtype must be 2 (bf16) or 0 (fp32)");
@@ -446,8 +448,11 @@ extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_pro
     if (rc) return rc;
     if ((probs[i].absmax_u8 != nullptr) != nested)
       return set_error(QB200_EUNSUPPORTED, "nf4_linear_group: all problems must be nested or all plain");
+    if (row_scales && reinterpret_cast<uintptr_t>(row_scales[i]) % 4 != 0)
+      return set_error(QB200_EINVAL, "nf4_linear_group_scaled: row scales must be 4-byte aligned fp32");
   }
-  gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), out_dtype == QB200_DTYPE_F32 ? 1 : 0, workspace, workspace_bytes};
+  gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), out_dtype == QB200_DTYPE_F32 ? 1 : 0, workspace, workspace_bytes,
+                    row_scales};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // forward with at most 16 tokens: warp-level skinny kernels (nf4_gemv.cu), SURVEY.md 8f-2 — with LoRA operands too (the
   // reference generates with the adapters attached: base GEMV + peft's two small matmuls; here the U . V^T term is the
@@ -457,12 +462,25 @@ extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_pro
     for (int i = 0; i < nprob; ++i) {
       const qb200_nf4_problem& q = probs[i];
       rc = launch_nf4_skinny(q.in, q.ld_in, q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_u8 ? nullptr : q.absmax_f32,
-                             q.bias, q.out, q.ld_out, int(M), int(N), int(K), q.U, q.ld_u, q.V, int(R), s);
+                             q.bias, q.out, q.ld_out, int(M), int(N), int(K), q.U, q.ld_u, q.V, int(R),
+                             row_scales ? row_scales[i] : nullptr, s);
       if (rc) return rc;
     }
     return 0;
   }
   return is_bwd ? gemm::launch_gemm<true>(g, s) : gemm::launch_gemm<false>(g, s);
+}
+
+extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M, int64_t N,
+                                      int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
+  return linear_group(is_bwd, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+}
+
+extern "C" int qb200_nf4_linear_group_scaled(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales,
+                                             int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
+                                             int64_t workspace_bytes, void* stream) {
+  if (!row_scales) return set_error(QB200_EINVAL, "nf4_linear_group_scaled: null row-scale array (NULL entries mean unscaled)");
+  return linear_group(is_bwd, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
 }
 
 extern "C" int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t K, int is_bwd) {

@@ -269,6 +269,10 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       if (p.nprob > 1) offs1 = __ldg(p.pr[1].offset);
       if (p.nprob > 2) offs2 = __ldg(p.pr[2].offset);
     }
+    // a row scale is the output of an earlier kernel, unlike the frozen NF4 state: scaled launches give up the prologue overlap
+    if (p.pr[0].row_scale != nullptr || (p.nprob > 1 && p.pr[1].row_scale != nullptr) ||
+        (p.nprob > 2 && p.pr[2].row_scale != nullptr))
+      ptx::grid_dep_wait();
     const int kblocks_per_row = p.K >> 6;
     int r;
     uint32_t st_base;
@@ -328,6 +332,8 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
     AbsmaxFetch<kNested> fetch;
     bool valid_cur = false;
     int pi_cur = 0;
+    const float* rs_ptr = nullptr;           // row scale of the current problem (null: unscaled)
+    float rs_cur = 1.0f;
     uint4 raw0 = make_uint4(0, 0, 0, 0), raw1 = make_uint4(0, 0, 0, 0);   // nibbles of the step this group handles next
     // Global loads of the group's next step (iterator already advanced).  Issued right AFTER the step's fence.proxy.async +
     // arrive.  Addresses advance incrementally (kNumGroups contraction steps per turn) and are recomputed only when the unit
@@ -342,6 +348,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       const int kb = u.kb0 + i;
       if (fresh) {
         pi_cur = p.group_sum ? seg : u.prob;
+        rs_ptr = p.pr[pi_cur].row_scale;
         wp_next = w_ptr(p.pr[pi_cur].packed, u.f0, kb);
         blk_next = blk_of(u.f0, kb);
         fresh = false;
@@ -356,7 +363,8 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       else
         valid_cur = (kb * kBlockC + r) < p.N && (u.f0 + (t >> 6) * 64) < p.K;
       fetch.issue(p.pr[pi_cur], blk_next, valid_cur);
-      raw0 = valid_cur ? __ldg(wp_next) : make_uint4(0, 0, 0, 0);
+      if (rs_ptr != nullptr) rs_cur = valid_cur ? __ldg(rs_ptr + (kTrans ? kb * kBlockC + r : u.f0 + r)) : 0.0f;
+      raw0 =valid_cur ? __ldg(wp_next) : make_uint4(0, 0, 0, 0);
       raw1 = valid_cur ? __ldg(wp_next + 1) : make_uint4(0, 0, 0, 0);
     };
     prefetch_step();
@@ -365,7 +373,8 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       const uint32_t empty_ph = ((g / kStages) & 1) ^ 1;
       if (i < u.nkb) {
         const float offset = pi_cur == 0 ? offs0 : (pi_cur == 1 ? offs1 : offs2);
-        const float am = fetch.resolve(s_code + pi_cur * 256, offset, valid_cur);
+        float am = fetch.resolve(s_code + pi_cur * 256, offset, valid_cur);
+        if (rs_ptr != nullptr) am = __fmul_rn(am, rs_cur);
         Nf4Table tab;
         build_table(am, tab);
         const uint32_t words[8] = {raw0.x, raw0.y, raw0.z, raw0.w, raw1.x, raw1.y, raw1.z, raw1.w};

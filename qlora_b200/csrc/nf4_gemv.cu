@@ -139,7 +139,7 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
                   const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
                   const float* __restrict__ absmax_f32, const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ y, int M,
                   int N, int K, const __nv_bfloat16* __restrict__ lora_u, int ld_u, const __nv_bfloat16* __restrict__ lora_v,
-                  int lora_r, int64_t ld_x, int64_t ld_y) {
+                  int lora_r, int64_t ld_x, int64_t ld_y, const float* __restrict__ row_scale) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   // [kWarps][NT * 8 tokens][512 B] x slabs, then 256 floats codebook; the slabs are re-used for the partial sums at the end
   uint8_t* slab_base = smem_raw;
@@ -191,6 +191,8 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
   for (int u = 0; u < kRing; ++u) fetch(b0 + 4 * kWarps * u, ring[u]);
   ptx::grid_dep_wait();
   stage(4 * warp);
+  // optional per-row weight scale (an earlier kernel's output: read after the wait); every block of this thread is in row n
+  const float rs = row_scale != nullptr ? __ldg(row_scale + n) : 1.0f;
   float offset = 0.0f;
   if (kNested) {
     for (int i = threadIdx.x; i < 256; i += 32 * kWarps) s_code[i] = __ldg(code256 + i);
@@ -223,6 +225,7 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
       const BlockRegs cur = ring[u];
       fetch(b + 4 * kWarps * kRing, ring[u]);
       float am = kNested ? nested_absmax(s_code[cur.code], cur.scale, offset) : cur.scale;
+      if (row_scale != nullptr) am = __fmul_rn(am, rs);
       if (b >= nblk) am = 0.0f;
       Table tab;
       build_table(am, tab);
@@ -294,7 +297,7 @@ static int launch_pdl(Kern kern, unsigned grid, unsigned block, int smem, cudaSt
 template <int NT, int kWarps, int kRing>
 static int launch_cfg(const void* x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256, const float* absmax2,
                       const float* offset, const float* absmax_f32, const void* bias, void* y, int M, int N, int K, const void* U,
-                      int ld_u, const void* V, int R, int64_t ld_x, int64_t ld_y, cudaStream_t stream) {
+                      int ld_u, const void* V, int R, int64_t ld_x, int64_t ld_y, const float* row_scale, cudaStream_t stream) {
   const unsigned grid = unsigned(N / kRows);
   constexpr int smem = kWarps * NT * 8 * kSlabRowBytes + 256 * int(sizeof(float));
   static_assert(smem <= 48 * 1024, "static opt-in not needed below 48 KB");
@@ -307,9 +310,9 @@ static int launch_cfg(const void* x, const uint8_t* packed, const uint8_t* absma
   const auto* vb = static_cast<const __nv_bfloat16*>(V);
   if (absmax_u8 != nullptr)
     return launch_pdl(nf4_skinny_kernel<NT, kWarps, kRing, true>, grid, 32 * kWarps, smem, stream, "nf4_skinny", xb, packed, absmax_u8,
-                      code256, absmax2, offset, no_f, bb, yb, M, N, K, ub, ld_u, vb, R, ld_x, ld_y);
+                      code256, absmax2, offset, no_f, bb, yb, M, N, K, ub, ld_u, vb, R, ld_x, ld_y, row_scale);
   return launch_pdl(nf4_skinny_kernel<NT, kWarps, kRing, false>, grid, 32 * kWarps, smem, stream, "nf4_skinny", xb, packed, no_u8, no_f,
-                    no_f, no_f, absmax_f32, bb, yb, M, N, K, ub, ld_u, vb, R, ld_x, ld_y);
+                    no_f, no_f, absmax_f32, bb, yb, M, N, K, ub, ld_u, vb, R, ld_x, ld_y, row_scale);
 }
 
 template <int N>
@@ -333,7 +336,8 @@ __global__ void __launch_bounds__(32 * kWarps, 4)
 nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
                        const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
                        const float* __restrict__ absmax_f32, const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ y,
-                       int N, int K, const __nv_bfloat16* __restrict__ lora_u, const __nv_bfloat16* __restrict__ lora_v, int lora_r) {
+                       int N, int K, const __nv_bfloat16* __restrict__ lora_u, const __nv_bfloat16* __restrict__ lora_v, int lora_r,
+                       const float* __restrict__ row_scale) {
   constexpr int kWarpSlab = kBuf * kSlabRowBytes;
   static_assert(kRing % kBuf == 0, "the slab of ring slot u is buffer u % kBuf");
   static_assert(32 * kWarps >= 16 * kRows, "the LoRA epilogue uses 16 lanes per weight row");
@@ -387,6 +391,7 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
     if (u < nsteps) stage(u, u);
     cp_async_commit();
   }
+  const float rs = row_scale != nullptr ? __ldg(row_scale + n) : 1.0f;   // as in nf4_skinny_kernel
   __syncthreads();
 
   float acc[2][4];
@@ -412,6 +417,7 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
       __syncwarp();
       BlockRegs& cur = ring[u];
       float am = kNested ? nested_absmax(s_code[cur.code], cur.scale, offset) : cur.scale;
+      if (row_scale != nullptr) am = __fmul_rn(am, rs);
       if (4 * (warp + kWarps * s) + t >= nblk) am = 0.0f;
       Table tab;
       build_table(am, tab);
@@ -474,7 +480,7 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
 template <int kWarps, int kRing, int kBuf>
 static int launch_1tok(const void* x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256, const float* absmax2,
                        const float* offset, const float* absmax_f32, const void* bias, void* y, int N, int K, const void* U,
-                       const void* V, int R, cudaStream_t stream) {
+                       const void* V, int R, const float* row_scale, cudaStream_t stream) {
   const unsigned grid = unsigned(N / kRows);
   constexpr int kSlabs = kWarps * kBuf * kSlabRowBytes;
   constexpr int kRed = (kWarps + 1) * kRows * int(sizeof(float));
@@ -487,21 +493,22 @@ static int launch_1tok(const void* x, const uint8_t* packed, const uint8_t* absm
   if (absmax_u8 != nullptr)
     return launch_pdl(nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, true>, grid, 32 * kWarps, smem, stream, "nf4_skinny_1tok", xb, packed,
                       absmax_u8, code256, absmax2, offset, no_f, bb, yb, N, K, static_cast<const __nv_bfloat16*>(U),
-                      static_cast<const __nv_bfloat16*>(V), R);
+                      static_cast<const __nv_bfloat16*>(V), R, row_scale);
   return launch_pdl(nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, false>, grid, 32 * kWarps, smem, stream, "nf4_skinny_1tok", xb, packed,
                     no_u8, no_f, no_f, no_f, absmax_f32, bb, yb, N, K, static_cast<const __nv_bfloat16*>(U),
-                    static_cast<const __nv_bfloat16*>(V), R);
+                    static_cast<const __nv_bfloat16*>(V), R, row_scale);
 }
 
 }  // namespace skinny
 
 // Internal: forward skinny GEMM, 16 tokens per launch (more tokens = more passes over the packed weights, which stay in L2);
-// optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); x / y / U may be column slices of wider row-major buffers (row
+// optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; x / y / U may be column slices of wider row-major buffers (row
 // pitches ld_x / ld_y / ld_u in elements, 0 = dense); caller has validated pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0,
 // R <= 64, 16-byte aligned x / U rows and V).
 int launch_nf4_skinny(const void* x, int64_t ld_x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
                       const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, void* y, int64_t ld_y,
-                      int M, int N, int K, const void* U, int64_t ld_u, const void* V, int R, cudaStream_t stream) {
+                      int M, int N, int K, const void* U, int64_t ld_u, const void* V, int R, const float* row_scale,
+                      cudaStream_t stream) {
   if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");
   if (R == 0) U = V = nullptr;
   if (ld_u == 0) ld_u = R;
@@ -515,13 +522,13 @@ int launch_nf4_skinny(const void* x, int64_t ld_x, const uint8_t* packed, const 
     void* yc = static_cast<__nv_bfloat16*>(y) + int64_t(m0) * ld_y;
     int rc;
     if (mc == 1)   // one token: row pitches do not matter
-      rc = skinny::launch_1tok<4, 4, 2>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, N, K, uc, V, R, stream);
+      rc = skinny::launch_1tok<4, 4, 2>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, N, K, uc, V, R, row_scale, stream);
     else if (mc <= 8)
       rc = skinny::launch_cfg<1, 4, 4>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, mc, N, K, uc, int(ld_u), V,
-                                       R, ld_x, ld_y, stream);
+                                       R, ld_x, ld_y, row_scale, stream);
     else
       rc = skinny::launch_cfg<2, 4, 4>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, mc, N, K, uc, int(ld_u), V,
-                                       R, ld_x, ld_y, stream);
+                                       R, ld_x, ld_y, row_scale, stream);
     if (rc) return rc;
   }
   return 0;

@@ -478,13 +478,15 @@ def _state_tensors(qs: QuantState, dev: torch.device):
 
 
 def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None, vs=None, outs=None,
-                     out_dtype: torch.dtype = torch.bfloat16):
+                     out_dtype: torch.dtype = torch.bfloat16, row_scales=None):
     """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group`).
 
     forward  (is_bwd=False): out_p = in_p . W_p^T (+bias_p) + U_p . V_p^T for every problem (the inputs may be one tensor);
                              returns the list of outputs.
     backward (is_bwd=True) : ONE output  sum_p (in_p . W_p + U_p . V_p), accumulated in the kernel; returns it.
     Inputs / U / outputs may be column slices of wider row-major buffers (row pitch passed through).
+    row_scales: None, or one fp32 [N] tensor (or None) per problem; W_p is then diag(row_scales[p]) . W_p, the scale folded
+    into the absmax of every NF4 block of the row (`qb200_nf4_linear_group_scaled`).
     """
     n = len(states)
     assert 1 <= n <= 3 and len(inputs) == n and len(packeds) == n
@@ -545,13 +547,31 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
             o = outs[i]
             assert o.shape == (m, f_out) and o.stride(1) == 1 and o.dtype == (torch.float32 if out_dtype == torch.float32 else torch.bfloat16)
             pr.out, pr.ld_out = o.data_ptr(), o.stride(0)
+    scales = None
+    if row_scales is not None:
+        assert len(row_scales) == n
+        scales = (ct.c_void_p * n)()
+        for i, sc in enumerate(row_scales):
+            if sc is None:
+                continue
+            assert sc.shape == (n_out,) and sc.dtype == torch.float32 and sc.device == dev, "row scale: fp32 [N] on the GPU"
+            if not sc.is_contiguous():
+                sc = sc.contiguous()
+                keep.append(sc)
+            scales[i] = sc.data_ptr()
     ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
-    what = ("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
+    what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
+            + ("_scaled" if scales is not None else ""))
     with torch.cuda.device(dev):
         ev = _event_begin()
-        check(lib.qb200_nf4_linear_group(int(is_bwd), n, ct.addressof(probs), r, m, n_out, k_in,
-                                         0 if out_dtype == torch.float32 else 2, ptr(ws), ws_bytes, stream_ptr(dev)), what)
+        if scales is None:
+            rc = lib.qb200_nf4_linear_group(int(is_bwd), n, ct.addressof(probs), r, m, n_out, k_in,
+                                            0 if out_dtype == torch.float32 else 2, ptr(ws), ws_bytes, stream_ptr(dev))
+        else:
+            rc = lib.qb200_nf4_linear_group_scaled(int(is_bwd), n, ct.addressof(probs), ct.addressof(scales), r, m, n_out, k_in,
+                                                   0 if out_dtype == torch.float32 else 2, ptr(ws), ws_bytes, stream_ptr(dev))
+        check(rc, what)
         _event_end(what, m * n, n_out, k_in, ev)
     return outs[0] if is_bwd else outs
 
@@ -613,3 +633,45 @@ def nf4_linear_bwd_dx_lora(dy2d: Tensor, packed: Tensor, quant_state: QuantState
                            out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
     """dX[M,K] = dY . W + U . Vt in one launch (U[M,r] bf16, Vt[r,K] bf16 = lora_A.weight)."""
     return _linear_ex(True, dy2d, packed, quant_state, None, u, vt, out_dtype=out_dtype)
+
+
+# --------------------------------------------------------------------------------------
+# DoRA over the NF4 base (weight-decomposed LoRA, Liu et al. 2024): the row norm of W + s.B.A without materialising W
+# --------------------------------------------------------------------------------------
+
+def weight_row_norm2(packed: Tensor, quant_state: QuantState) -> Tensor:
+    """||W_f||^2 for every row f of the frozen NF4 weight: the bf16 weight `dequantize_4bit` returns, squared and summed in
+    fp32; fp32 [N].  Cached on the QuantState (the base never changes), so call it once at setup: inside a CUDA-graph
+    capture a missing cache is an error, not a lazy allocation."""
+    cached = getattr(quant_state, "row_norm2", None)
+    if cached is not None:
+        return cached
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("weight_row_norm2: compute the row norms of a frozen base before capturing a CUDA graph")
+    w = dequantize_4bit(packed.reshape(-1, 1), quant_state)     # [N, K] bf16 (the [1, n/2] view is not transposed back)
+    norm2 = torch.empty(w.shape[0], dtype=torch.float32, device=w.device)
+    for r0 in range(0, w.shape[0], 2048):                       # fp32 copies of 2048 rows at a time
+        norm2[r0:r0 + 2048] = w[r0:r0 + 2048].float().square().sum(1)
+    quant_state.row_norm2 = norm2
+    return norm2
+
+
+def dora_weight_norm(packeds, states, lora_as, lora_bs, scaling: float):
+    """DoRA's weight norm n_f = ||W_f + s (B A)_f||_2 (fp32 [N], no gradient) for 1..3 frozen NF4 weights of one shape,
+    from the expansion
+        n^2 = ||W_f||^2 + 2 s sum_j B[f, j] P[j, f] + s^2 (B G B^T)_ff,   P = A . W^T [r, N],  G = A . A^T [r, r],
+    with ||W_f||^2 cached per base (`weight_row_norm2`), P from ONE launch of the fused forward with the adapters A_p as r-token
+    inputs, and the rest small fp32 ops.  Single tensors or lists (q/k/v, gate/up) are accepted; returns the same form."""
+    single = isinstance(states, QuantState)
+    if single:
+        packeds, states, lora_as, lora_bs = [packeds], [states], [lora_as], [lora_bs]
+    with torch.no_grad():
+        ps = nf4_linear_group(False, [a.detach() for a in lora_as], list(packeds), list(states), out_dtype=torch.float32)
+        norms = []
+        for packed, qs, a, b, p in zip(packeds, states, lora_as, lora_bs, ps):
+            a32, b32 = a.detach().float(), b.detach().float()
+            cross = (b32 * p.t()).sum(1)
+            quad = ((b32 @ (a32 @ a32.t())) * b32).sum(1)
+            n2 = weight_row_norm2(packed, qs) + (2.0 * scaling) * cross + (scaling * scaling) * quad
+            norms.append(n2.clamp_min_(0.0).sqrt_())
+    return norms[0] if single else norms

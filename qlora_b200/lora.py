@@ -251,3 +251,163 @@ def lora_linear4bit_group(x: torch.Tensor, bases, lora_as, lora_bs, scaling: flo
     xl = [None] * n if x_loras is None else list(x_loras)
     states = tuple(b.weight.quant_state for b in bases)
     return LoraGroupMatMul4Bit.apply(x, float(scaling), states, n, *xl, *[b.weight.t() for b in bases], *lora_as, *lora_bs)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# DoRA over the NF4 base ("QDoRA"; Liu et al., ICML 2024; peft `use_dora=True` on a Linear4bit)
+# ----------------------------------------------------------------------------------------------------------------------
+# With the detached weight norm n = ||W + s.B.A||_row and c = m / n (fp32), peft's DoraLinearLayer computes
+#     no dropout : y = c * (x . W^T + s (x . A^T) . B^T)
+#     dropout    : y = x . W^T + (c - 1) * (xd . W^T) + c * s (xd . A^T) . B^T,    xd = drop(x)
+# A per-output-feature scale of W is a scale of the absmax of every NF4 block of that row, so the kernels take c as a row
+# scale: no dropout is ONE fused launch  y = x . (diag(c) W)^T + U . (diag(c) B)^T;  with dropout
+# y = (x - xd) . W^T + c * Q,  Q = xd . W^T + U . B^T  (one fused LoRA launch + one plain launch).  Backward:
+#     dQ = dy * c,  G = s dQ . B = s dy . (diag(c) B),  dA = G^T . xd,  dB = dQ^T . U,  dm = sum_t dy * Q / n
+#     no dropout : dx  = dy . diag(c) W + G . A                           (one launch, row scale c)
+#     dropout    : dx  = dy . W,   dxd = dy . diag(c - 1) W + G . A      (row scale c - 1; dxd flows back through the mask)
+
+
+def _accumulate_or_return(param: torch.Tensor, grad: torch.Tensor):
+    """`grad` as the gradient of `param`, or added in place to its existing buffer (see ACCUMULATE_ADAPTER_GRADS_IN_PLACE)."""
+    g = param.grad
+    if ACCUMULATE_ADAPTER_GRADS_IN_PLACE and g is not None and g.dtype == grad.dtype and g.shape == grad.shape:
+        g.add_(grad)
+        return None
+    return grad
+
+
+class DoraMatMul4Bit(torch.autograd.Function):
+    """n = 1..3 DoRA-wrapped Linear4bit of one shape applied to ONE input (q/k/v, gate/up: one launch per direction)."""
+
+    @staticmethod
+    def forward(ctx, x, scaling: float, states, n: int, *tensors):
+        # tensors = x_lora[0..n) (None: no dropout), packed_t[0..n), lora_a[0..n), lora_b[0..n), magnitude[0..n)
+        x_loras, packeds = tensors[:n], list(tensors[n:2 * n])
+        lora_as, lora_bs, mags = tensors[2 * n:3 * n], tensors[3 * n:4 * n], tensors[4 * n:5 * n]
+        states = list(states)
+        x2d = _as_bf16_2d(x)
+        r = lora_as[0].shape[0]
+        split = x_loras[0] is not None
+        norms = F.dora_weight_norm(packeds, states, list(lora_as), list(lora_bs), scaling)
+        cs = [m.detach().float() / nrm for m, nrm in zip(mags, norms)]
+        out_dtype = torch.float32 if x.dtype == torch.float32 else torch.bfloat16
+        if not split:
+            a_cat = _adjacent_rows(lora_as) if n > 1 else lora_as[0]
+            if a_cat is None:
+                a_cat = torch.cat(list(lora_as), 0)
+            u_cat = _project(x2d, a_cat, scaling)
+            us = [u_cat[:, i * r:(i + 1) * r] for i in range(n)]
+            xls = [x2d] * n
+            vs = [(b.float() * c[:, None]).to(torch.bfloat16) for b, c in zip(lora_bs, cs)]    # diag(c) B
+            ys = F.nf4_linear_group(False, [x2d] * n, packeds, states, us=us, vs=vs, out_dtype=out_dtype, row_scales=cs)
+            qs_saved = ys                                            # Q = y / c: dm = sum_t dy * y / (c n)
+        else:
+            xls = [_as_bf16_2d(t) for t in x_loras]
+            us = [_project(xls[i], lora_as[i], scaling) for i in range(n)]
+            qs_saved = F.nf4_linear_group(False, xls, packeds, states, us=us, vs=[b.contiguous() for b in lora_bs])
+            ps = F.nf4_linear_group(False, [x2d - xl for xl in xls], packeds, states)
+            ys = [torch.addcmul(p.float(), q.float(), c).to(out_dtype) for p, q, c in zip(ps, qs_saved, cs)]
+        ctx.save_for_backward(*(xls if split else [x2d]), *us, *packeds, *lora_as, *lora_bs, *norms, *cs, *qs_saved)
+        ctx.params = (tuple(lora_as), tuple(lora_bs), tuple(mags))
+        ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, split
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if split else None
+        n_out = states[0].shape[0]
+        return tuple(y.view(*x.shape[:-1], n_out) for y in ys)
+
+    @staticmethod
+    def backward(ctx, *grad_ys):
+        n, split, s = ctx.n, ctx.split, ctx.scaling
+        saved = list(ctx.saved_tensors)
+        nx = n if split else 1
+        xls = saved[:nx] if split else [saved[0]] * n
+        rest = saved[nx:]
+        us, packeds, lora_as, lora_bs, norms, cs, qs_saved = (rest[i * n:(i + 1) * n] for i in range(7))
+        g2ds = [_as_bf16_2d(g) for g in grad_ys]
+        r = lora_as[0].shape[0]
+        # G_p = s (dy_p * c_p) . B_p = s dy_p . (diag(c_p) B_p), written side by side for one dA GEMM
+        g_cat = torch.empty((g2ds[0].shape[0], n * r), dtype=torch.bfloat16, device=g2ds[0].device)
+        gs = [_scaled_mm(g2ds[i], (lora_bs[i].float() * cs[i][:, None]).to(torch.bfloat16), s, out=g_cat[:, i * r:(i + 1) * r])
+              for i in range(n)]
+        out_dtype = torch.float32 if ctx.x_dtype == torch.float32 else torch.bfloat16
+        grad_x = None
+        grad_xls = [None] * n
+        if split:
+            if ctx.needs_input_grad[0]:
+                grad_x = F.nf4_linear_group(True, g2ds, list(packeds), ctx.states, out_dtype=out_dtype).view(ctx.x_shape)
+            for i in range(n):
+                if ctx.needs_input_grad[4 + i]:
+                    shape, dtype = ctx.xl_meta[i]
+                    grad_xls[i] = F.nf4_linear_group(True, [g2ds[i]], [packeds[i]], [ctx.states[i]], us=[gs[i]],
+                                                     vs=[lora_as[i].contiguous()], row_scales=[cs[i] - 1.0],
+                                                     out_dtype=torch.float32 if dtype == torch.float32 else torch.bfloat16).view(shape)
+        elif ctx.needs_input_grad[0]:
+            grad_x = F.nf4_linear_group(True, g2ds, list(packeds), ctx.states, us=gs, vs=[a.contiguous() for a in lora_as],
+                                        out_dtype=out_dtype, row_scales=list(cs)).view(ctx.x_shape)
+        pa, pb, pm = ctx.params
+        if split or n == 1:
+            grad_as = [_adapter_grad(pa[i], gs[i].t(), xls[i]) for i in range(n)]
+        else:
+            ga_cat = torch.mm(g_cat.t(), xls[0])
+            grad_as = [_accumulate_or_return(pa[i], ga_cat[i * r:(i + 1) * r]) for i in range(n)]
+        grad_bs, grad_ms = [], []
+        for i in range(n):
+            grad_bs.append(_accumulate_or_return(pb[i], (torch.mm(g2ds[i].t(), us[i]).float() * cs[i][:, None]).to(pb[i].dtype)))
+            dq = (grad_ys[i].reshape(-1, grad_ys[i].shape[-1]).float() * qs_saved[i].float()).sum(0)
+            dm = dq / (norms[i] * cs[i]) if not split else dq / norms[i]
+            grad_ms.append(_accumulate_or_return(pm[i], dm.to(pm[i].dtype)))
+        return (grad_x, None, None, None, *grad_xls, *([None] * n), *grad_as, *grad_bs, *grad_ms)
+
+
+def _dora_fusable(x, base, lora_a, lora_b, magnitude) -> bool:
+    return _fusable(x, base, lora_a, lora_b) and magnitude.dtype == lora_a.dtype and magnitude.shape == (base.out_features,)
+
+
+def dora_linear4bit_peft(x, base, lora_a, lora_b, magnitude, scaling: float, x_lora=None):
+    """peft's `lora.Linear` + `DoraLinearLayer` forward for a Linear4bit base, restated on the library's unfused kernels:
+    the whole NF4 weight is dequantized every call for the norm and, with dropout, the base GEMM runs a second time on the
+    dropped input.  The reference the fused path is checked and timed against, and its fallback."""
+    result = base(x)
+    weight = F.dequantize_4bit(base.weight.data, base.weight.quant_state).to(lora_a.dtype)
+    lora_weight = lora_b @ lora_a
+    weight_norm = torch.linalg.norm(weight + scaling * lora_weight.detach(), dim=1).to(weight.dtype).detach()
+    mag_norm_scale = (magnitude / weight_norm).view(1, -1)
+    xl = x if x_lora is None else x_lora
+    xl = xl.to(lora_a.dtype)
+    lora_result = torch.nn.functional.linear(torch.nn.functional.linear(xl, lora_a), lora_b)
+    if x_lora is None:
+        base_result = result if base.bias is None else result - base.bias
+    else:
+        base_result = torch.nn.functional.linear(xl, weight)
+    result_dora = (mag_norm_scale - 1) * base_result + mag_norm_scale * lora_result * scaling
+    return result + result_dora.to(result.dtype)
+
+
+def dora_linear4bit(x: torch.Tensor, base, lora_a: torch.Tensor, lora_b: torch.Tensor, magnitude: torch.Tensor, scaling: float,
+                    x_lora: torch.Tensor | None = None) -> torch.Tensor:
+    """DoRA over a quantized `Linear4bit` base (peft `use_dora=True`), fused: the magnitude `m` rescales the rows of W inside
+    the NF4 kernels.  `x_lora` is the dropped input of the adapter branch (None: no dropout / eval).  Falls back to
+    `dora_linear4bit_peft` where `lora_linear4bit` falls back (rank, bias, dtype, shape)."""
+    if _dora_fusable(x, base, lora_a, lora_b, magnitude):
+        return DoraMatMul4Bit.apply(x, float(scaling), (base.weight.quant_state,), 1, x_lora, base.weight.t(), lora_a, lora_b,
+                                    magnitude)[0]
+    return dora_linear4bit_peft(x, base, lora_a, lora_b, magnitude, scaling, x_lora)
+
+
+def dora_linear4bit_group(x: torch.Tensor, bases, lora_as, lora_bs, magnitudes, scaling: float, x_loras=None):
+    """`dora_linear4bit` for 2-3 Linear4bit of one shape on one input (q/k/v, gate/up): one launch per direction for the
+    GEMMs, one launch for their weight norms.  Falls back to per-linear calls when the group does not qualify."""
+    n = len(bases)
+    shapes = {tuple(b.weight.quant_state.shape) if getattr(b.weight, "quant_state", None) is not None else None for b in bases}
+    ranks = {a.shape[0] for a in lora_as}
+    nested = {b.weight.quant_state.nested for b in bases if getattr(b.weight, "quant_state", None) is not None}
+    ok = (2 <= n <= 3 and len(shapes) == 1 and None not in shapes and len(ranks) == 1 and len(nested) == 1
+          and all(_dora_fusable(x, bases[i], lora_as[i], lora_bs[i], magnitudes[i]) for i in range(n))
+          and (x_loras is None or all(t is not None for t in x_loras)))
+    if not ok:
+        return tuple(dora_linear4bit(x, bases[i], lora_as[i], lora_bs[i], magnitudes[i], scaling,
+                                     None if x_loras is None else x_loras[i]) for i in range(n))
+    xl = [None] * n if x_loras is None else list(x_loras)
+    states = tuple(b.weight.quant_state for b in bases)
+    return DoraMatMul4Bit.apply(x, float(scaling), states, n, *xl, *[b.weight.t() for b in bases], *lora_as, *lora_bs,
+                                *magnitudes)

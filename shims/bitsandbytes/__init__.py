@@ -14,6 +14,7 @@ if _root not in _sys.path:
 import qlora_b200 as _impl  # noqa: E402
 from qlora_b200 import MatMul4Bit, matmul_4bit  # noqa: E402,F401
 from qlora_b200 import lora_linear4bit, lora_linear4bit_group  # noqa: E402,F401  (extensions: fused LoRA step, SURVEY.md 8f-1)
+from qlora_b200 import dora_linear4bit, dora_linear4bit_group, dora_linear4bit_peft  # noqa: E402,F401  (extensions: fused QDoRA)
 from qlora_b200 import functional, nn, optim  # noqa: E402,F401
 
 __version__ = _impl.__version__
