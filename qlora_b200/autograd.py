@@ -55,23 +55,11 @@ class MatMul4Bit(torch.autograd.Function):
                 return torch.empty(A.shape[:-1] + B_shape[1:], dtype=A.dtype, device=A.device)
             return torch.empty(A.shape[:-1] + B_shape[:1], dtype=A.dtype, device=A.device)
 
-        n_out = quant_state.shape[0]
-        fused = ctx.io_dtype is None and USE_FUSED and B.shape[0] == 1 and F.fused_supported(quant_state, A.dtype)
-        if ctx.io_dtype is not None:
-            fused = True
-            a2d = A.reshape(-1, A.shape[-1]).to(torch.bfloat16)
+        fused = ctx.io_dtype is not None or (USE_FUSED and B.shape[0] == 1 and F.fused_supported(quant_state, A.dtype))
+        if fused:
             b = bias if (bias is None or bias.dtype == torch.bfloat16) else bias.to(torch.bfloat16)
-            y = F.nf4_linear_fwd(a2d.contiguous(), B, quant_state, b, out_dtype=torch.float32)
-            output = y.view(*A.shape[:-1], n_out)
-        elif fused:
-            a2d = A.reshape(-1, A.shape[-1])
-            if not a2d.is_contiguous():
-                a2d = a2d.contiguous()
-            b = bias
-            if b is not None and b.dtype != torch.bfloat16:
-                b = b.to(torch.bfloat16)
-            y = F.nf4_linear_fwd(a2d, B, quant_state, b)
-            output = y.view(*A.shape[:-1], n_out)
+            y = F.nf4_linear_fwd(F.as_bf16_2d(A), B, quant_state, b, out_dtype=F.out_dtype_for(A.dtype))
+            output = y.view(*A.shape[:-1], quant_state.shape[0])
         else:
             output = torch.nn.functional.linear(A, _unfused_weight(B, quant_state, A.dtype).t(), bias)
         if out is not None:
@@ -98,16 +86,9 @@ class MatMul4Bit(torch.autograd.Function):
         if req_gradBias:
             # sum over every leading dim (upstream sums dim 0 only, which is wrong for 3-D inputs)
             grad_bias = grad_output.reshape(-1, grad_output.shape[-1]).sum(0, dtype=ctx.dtype_bias)
-        if req_gradA and ctx.io_dtype is not None:
-            g2d = grad_output.reshape(-1, grad_output.shape[-1]).to(torch.bfloat16).contiguous()
-            dx = F.nf4_linear_bwd_dx(g2d, B, ctx.state, out_dtype=torch.float32)
-            grad_A = dx.view(*grad_output.shape[:-1], ctx.state.shape[1])
-        elif req_gradA:
-            if ctx.fused and grad_output.dtype == torch.bfloat16:
-                g2d = grad_output.reshape(-1, grad_output.shape[-1])
-                if not g2d.is_contiguous():
-                    g2d = g2d.contiguous()
-                dx = F.nf4_linear_bwd_dx(g2d, B, ctx.state)
+        if req_gradA:
+            if ctx.fused and (ctx.io_dtype is not None or grad_output.dtype == torch.bfloat16):
+                dx = F.nf4_linear_bwd_dx(F.as_bf16_2d(grad_output), B, ctx.state, out_dtype=F.out_dtype_for(ctx.dtype_A))
                 grad_A = dx.view(*grad_output.shape[:-1], ctx.state.shape[1])
             else:
                 grad_A = torch.matmul(grad_output, _unfused_weight(B, ctx.state, grad_output.dtype).t())

@@ -436,6 +436,20 @@ def fused_supported(quant_state: QuantState, compute_dtype: torch.dtype) -> bool
     return True
 
 
+def as_bf16_2d(t: Tensor) -> Tensor:
+    """`t` as the contiguous bf16 [rows, last dim] matrix the fused kernels read (cast and copied only where needed)."""
+    t2 = t.reshape(-1, t.shape[-1])
+    if t2.dtype != torch.bfloat16:
+        t2 = t2.to(torch.bfloat16)
+    return t2 if t2.is_contiguous() else t2.contiguous()
+
+
+def out_dtype_for(in_dtype: torch.dtype) -> torch.dtype:
+    """What a fused launch writes for activations of `in_dtype`: fp32 for fp32 (the kernel's epilogue widens the bf16-rounded
+    result, as `Linear4bit.forward` returns fp32 for fp32 input), else bf16."""
+    return torch.float32 if in_dtype == torch.float32 else torch.bfloat16
+
+
 def _event_begin():
     LAUNCH_COUNTER[0] += 1
     if EVENT_LOG is None:

@@ -20,10 +20,11 @@ passed as a second input.  Forward is unchanged (U comes from x_lora); in backwa
 must go through the dropout mask, so it is returned as the gradient of `x_lora` (G . A, one extra skinny GEMM) and the
 fused dX launch carries the base term only.
 
-Linears that share their input and shape (q/k/v, gate/up) run as ONE grouped launch per direction
-(`lora_linear4bit_group`): the three (two) forward GEMMs side by side, the backward as one long contraction
-dX = sum_p (dY_p . W_p + G_p . A_p) accumulated in the same accumulators — no separate accumulation of the input gradient — and the
-`x . A_p^T` projections batched into one GEMM.
+One autograd function, `LoraMatMul4Bit`, covers 1..3 linears on one input.  Linears that share their input and shape
+(q/k/v, gate/up; `lora_linear4bit_group`) run as ONE grouped launch per direction: the three (two) forward GEMMs side by
+side, the backward as one long contraction dX = sum_p (dY_p . W_p + G_p . A_p) accumulated in the same accumulators — no
+separate accumulation of the input gradient — and the `x . A_p^T` projections batched into one GEMM.  A single linear
+(`lora_linear4bit`) is the same call with one problem.
 
 fp32 activations (the reference casts its norms to fp32, qlora.py:400-401, so `Linear4bit.forward` sees fp32 in and
 returns fp32): the input is cast to bf16 once per call (once per GROUP for q/k/v) and the kernel's epilogue writes the
@@ -85,54 +86,42 @@ def _adjacent_rows(ts) -> torch.Tensor | None:
     return torch.as_strided(t0.detach(), (rows, t0.shape[1]), (t0.shape[1], 1), t0.storage_offset())
 
 
-def _as_bf16_2d(t: torch.Tensor) -> torch.Tensor:
-    t2 = t.reshape(-1, t.shape[-1])
-    if t2.dtype != torch.bfloat16:
-        t2 = t2.to(torch.bfloat16)
-    return t2 if t2.is_contiguous() else t2.contiguous()
+def _split(seq, n: int, k: int):
+    """The first k * n items of `seq` as k lists of n: the per-linear groups of an autograd function's variadic inputs, its
+    saved tensors or its `needs_input_grad` flags."""
+    return [list(seq[i * n:(i + 1) * n]) for i in range(k)]
 
 
-class LoraMatMul4Bit(torch.autograd.Function):
-    """y = x . W^T + scaling * (x_lora . A^T) . B^T for ONE frozen NF4 Linear4bit (x_lora = None: the same tensor as x)."""
+def _apply(fn, x, bases, scaling: float, x_loras, *per_linear):
+    """`fn.apply` on n = len(bases) linears, its variadic inputs in the order `fn.forward` splits them: x_lora[0..n) (None:
+    no dropout), packed_t[0..n), then each list of `per_linear` (lora_a[0..n), lora_b[0..n), ...)."""
+    n = len(bases)
+    x_loras = [None] * n if x_loras is None else x_loras
+    return fn.apply(x, float(scaling), tuple(b.weight.quant_state for b in bases), n, *x_loras, *[b.weight.t() for b in bases],
+                    *[t for ts in per_linear for t in ts])
 
-    @staticmethod
-    def forward(ctx, x, x_lora, packed_t, lora_a, lora_b, scaling: float, quant_state: F.QuantState):
-        x2d = _as_bf16_2d(x)
-        xl2d = x2d if x_lora is None else _as_bf16_2d(x_lora)
-        u = _project(xl2d, lora_a, scaling)
-        out_dtype = torch.float32 if x.dtype == torch.float32 else torch.bfloat16
-        y = F.nf4_linear_fwd_lora(x2d, packed_t, quant_state, u, lora_b.contiguous(), out_dtype=out_dtype)
-        ctx.save_for_backward(xl2d, u, packed_t, lora_a, lora_b)
-        ctx.adapters = (lora_a, lora_b)     # the Parameter objects themselves (their .grad buffers, see _adapter_grad)
-        ctx.state = quant_state
-        ctx.scaling = scaling
-        ctx.x_shape = x.shape
-        ctx.x_dtype = x.dtype
-        ctx.split_lora = x_lora is not None
-        ctx.xl_meta = None if x_lora is None else (x_lora.shape, x_lora.dtype)
-        return y.view(*x.shape[:-1], quant_state.shape[0])
 
-    @staticmethod
-    def backward(ctx, grad_y):
-        xl2d, u, packed_t, lora_a, lora_b = ctx.saved_tensors
-        g2d = _as_bf16_2d(grad_y)
-        g = _scaled_mm(g2d, lora_b, ctx.scaling)   # [M, r]
-        grad_x = grad_xl = grad_a = grad_b = None
-        out_dtype = torch.float32 if ctx.x_dtype == torch.float32 else torch.bfloat16
-        if ctx.split_lora:
-            # dropout on the LoRA branch: its input gradient goes back through the mask, the base term does not
-            if ctx.needs_input_grad[0]:
-                grad_x = F.nf4_linear_bwd_dx(g2d, packed_t, ctx.state, out_dtype=out_dtype).view(ctx.x_shape)
-            if ctx.needs_input_grad[1]:
-                shape, dtype = ctx.xl_meta
-                grad_xl = torch.mm(g, lora_a).to(dtype).view(shape)
-        elif ctx.needs_input_grad[0]:
-            grad_x = F.nf4_linear_bwd_dx_lora(g2d, packed_t, ctx.state, g, lora_a.contiguous(), out_dtype=out_dtype).view(ctx.x_shape)
-        if ctx.needs_input_grad[3]:
-            grad_a = _adapter_grad(ctx.adapters[0], g.t(), xl2d)       # [r, K]
-        if ctx.needs_input_grad[4]:
-            grad_b = _adapter_grad(ctx.adapters[1], g2d.t(), u)        # [N, r]
-        return grad_x, grad_xl, None, grad_a, grad_b, None, None
+def _project_inputs(x2d: torch.Tensor, x_loras, lora_as, scaling: float):
+    """(x_lora_p, U_p = scaling * x_lora_p . A_p^T) for every adapter, x_lora_p as bf16 [M, K].  Without dropout every x_lora_p
+    is x and ONE projection U_cat = scaling * x . [A_0; A_1; ..]^T is sliced into the U_p.  A single adapter is projected as it
+    is: a cat of one non-contiguous A would be a contiguous copy, which moves a <= 16-token step onto the library's projection."""
+    if x_loras[0] is not None:
+        xls = [F.as_bf16_2d(t) for t in x_loras]
+        return xls, [_project(xl, a, scaling) for xl, a in zip(xls, lora_as)]
+    n, r = len(lora_as), lora_as[0].shape[0]
+    a_cat = lora_as[0] if n == 1 else _adjacent_rows(lora_as)
+    if a_cat is None:
+        a_cat = torch.cat(lora_as, 0)
+    u_cat = _project(x2d, a_cat, scaling)
+    return [x2d] * n, [u_cat[:, i * r:(i + 1) * r] for i in range(n)]
+
+
+def _project_grads(g2ds, vs, scaling: float):
+    """G_p = scaling * dY_p . V_p ([M, r] each), written side by side into one [M, n r] buffer G_cat for a single dA GEMM;
+    returns (G_cat, [G_p])."""
+    r = vs[0].shape[1]
+    g_cat = torch.empty((g2ds[0].shape[0], len(vs) * r), dtype=torch.bfloat16, device=g2ds[0].device)
+    return g_cat, [_scaled_mm(g, v, scaling, out=g_cat[:, i * r:(i + 1) * r]) for i, (g, v) in enumerate(zip(g2ds, vs))]
 
 
 def _fusable(x, base, lora_a, lora_b) -> bool:
@@ -142,75 +131,51 @@ def _fusable(x, base, lora_a, lora_b) -> bool:
             and F.lora_fused_supported(qs, torch.bfloat16, lora_a.shape[0]))
 
 
-def lora_linear4bit(x: torch.Tensor, base, lora_a: torch.Tensor, lora_b: torch.Tensor, scaling: float,
-                    x_lora: torch.Tensor | None = None) -> torch.Tensor:
-    """`base(x) + (x_lora @ lora_a.T @ lora_b.T) * scaling` for a quantized `Linear4bit` base (no bias), fused.
-
-    `x_lora` is the LoRA branch's input when it differs from `x` (peft applies dropout to it); None = `x`.
-    Falls back to the two-step form (still on the GPU kernels) when the fused kernel does not cover the case
-    (fp16 compute dtype, rank not a multiple of 8 or > 64, bias present, unsupported shape)."""
-    if _fusable(x, base, lora_a, lora_b):
-        return LoraMatMul4Bit.apply(x, x_lora, base.weight.t(), lora_a, lora_b, float(scaling), base.weight.quant_state)
-    result = base(x)
-    xl = x if x_lora is None else x_lora
-    upd = torch.nn.functional.linear(torch.nn.functional.linear(xl.to(lora_a.dtype), lora_a), lora_b) * scaling
-    return result + upd.to(result.dtype)
+def _group_fusable(x, bases, lora_as, lora_bs, x_loras) -> bool:
+    """Whether 1..3 adapter-wrapped Linear4bit on the input `x` run as ONE fused call: the fused kernel covers each of them,
+    and they share one weight shape, one rank and one quantization form (all nested or all plain), with a dropout input for
+    every linear or for none."""
+    if not (1 <= len(bases) <= 3 and all(_fusable(x, b, a, bb) for b, a, bb in zip(bases, lora_as, lora_bs))):
+        return False
+    states = [b.weight.quant_state for b in bases]
+    return (len({tuple(qs.shape) for qs in states}) == 1 and len({a.shape[0] for a in lora_as}) == 1
+            and len({qs.nested for qs in states}) == 1 and (x_loras is None or all(t is not None for t in x_loras)))
 
 
-class LoraGroupMatMul4Bit(torch.autograd.Function):
-    """n = 2 or 3 LoRA-wrapped Linear4bit of one shape applied to ONE input: one fused launch per direction."""
+class LoraMatMul4Bit(torch.autograd.Function):
+    """y_p = x . W_p^T + scaling * (x_lora_p . A_p^T) . B_p^T for n = 1..3 LoRA-wrapped Linear4bit of one shape applied to ONE
+    input (q/k/v, gate/up: one fused launch per direction).  x_lora_p = None for every p: no dropout, the adapters read x."""
 
     @staticmethod
     def forward(ctx, x, scaling: float, states, n: int, *tensors):
-        # tensors = x_lora[0..n) (None: no dropout), packed_t[0..n), lora_a[0..n), lora_b[0..n)
-        x_loras, packeds = tensors[:n], tensors[n:2 * n]
-        lora_as, lora_bs = tensors[2 * n:3 * n], tensors[3 * n:4 * n]
-        x2d = _as_bf16_2d(x)
-        r = lora_as[0].shape[0]
-        split = x_loras[0] is not None
-        if not split:   # one projection for all adapters: U_cat = scaling * x . [A_0; A_1; ..]^T
-            a_cat = _adjacent_rows(lora_as)
-            if a_cat is None:
-                a_cat = torch.cat([a for a in lora_as], 0)
-            u_cat = _project(x2d, a_cat, scaling)
-            us = [u_cat[:, i * r:(i + 1) * r] for i in range(n)]
-            xls = [x2d] * n
-        else:
-            xls = [_as_bf16_2d(t) for t in x_loras]
-            us = [_project(xls[i], lora_as[i], scaling) for i in range(n)]
-        out_dtype = torch.float32 if x.dtype == torch.float32 else torch.bfloat16
-        ys = F.nf4_linear_group(False, [x2d] * n, list(packeds), list(states), us=us, vs=[b.contiguous() for b in lora_bs],
-                                out_dtype=out_dtype)
-        ctx.save_for_backward(*(xls if split else [x2d]), *us, *packeds, *lora_as, *lora_bs)
-        ctx.adapters = (tuple(lora_as), tuple(lora_bs))   # the Parameter objects themselves (their .grad buffers)
-        ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, split
+        x_loras, packeds, lora_as, lora_bs = _split(tensors, n, 4)
+        x2d = F.as_bf16_2d(x)
+        xls, us = _project_inputs(x2d, x_loras, lora_as, scaling)
+        ys = F.nf4_linear_group(False, [x2d] * n, packeds, list(states), us=us, vs=[b.contiguous() for b in lora_bs],
+                                out_dtype=F.out_dtype_for(x.dtype))
+        ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs)
+        ctx.adapters = (lora_as, lora_bs)   # the Parameter objects themselves (their .grad buffers, see _adapter_grad)
+        ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, x_loras[0] is not None
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
-        ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if split else None
+        ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if ctx.split else None
         n_out = states[0].shape[0]
         return tuple(y.view(*x.shape[:-1], n_out) for y in ys)
 
     @staticmethod
     def backward(ctx, *grad_ys):
         n, split = ctx.n, ctx.split
-        saved = list(ctx.saved_tensors)
-        nx = n if split else 1
-        xls = saved[:nx] if split else [saved[0]] * n
-        us = saved[nx:nx + n]
-        packeds = saved[nx + n:nx + 2 * n]
-        lora_as = saved[nx + 2 * n:nx + 3 * n]
-        lora_bs = saved[nx + 3 * n:nx + 4 * n]
-        g2ds = [_as_bf16_2d(g) for g in grad_ys]
-        r = lora_as[0].shape[0]
-        g_cat = torch.empty((g2ds[0].shape[0], n * r), dtype=torch.bfloat16, device=g2ds[0].device)
-        gs = [_scaled_mm(g2ds[i], lora_bs[i], ctx.scaling, out=g_cat[:, i * r:(i + 1) * r]) for i in range(n)]   # [M, r] slices
-        out_dtype = torch.float32 if ctx.x_dtype == torch.float32 else torch.bfloat16
+        xls, us, packeds, lora_as, lora_bs = _split(ctx.saved_tensors, n, 5)
+        need_xl, _, need_a, need_b = _split(ctx.needs_input_grad[4:], n, 4)
+        g2ds = [F.as_bf16_2d(g) for g in grad_ys]
+        g_cat, gs = _project_grads(g2ds, lora_bs, ctx.scaling)
+        out_dtype = F.out_dtype_for(ctx.x_dtype)
         grad_x = None
         grad_xls = [None] * n
         if split:
             if ctx.needs_input_grad[0]:
                 grad_x = F.nf4_linear_group(True, g2ds, packeds, list(ctx.states), out_dtype=out_dtype).view(ctx.x_shape)
             for i in range(n):
-                if ctx.needs_input_grad[4 + i]:
+                if need_xl[i]:
                     shape, dtype = ctx.xl_meta[i]
                     grad_xls[i] = torch.mm(gs[i], lora_as[i]).to(dtype).view(shape)
         elif ctx.needs_input_grad[0]:
@@ -218,8 +183,8 @@ class LoraGroupMatMul4Bit(torch.autograd.Function):
             grad_x = F.nf4_linear_group(True, g2ds, packeds, list(ctx.states), us=gs, vs=[a.contiguous() for a in lora_as],
                                         out_dtype=out_dtype).view(ctx.x_shape)
         pa, pb = ctx.adapters
-        if split:
-            grad_as = [_adapter_grad(pa[i], gs[i].t(), xls[i]) for i in range(n)]
+        if split or n == 1:
+            grad_as = [_adapter_grad(pa[i], gs[i].t(), xls[i]) if need_a[i] else None for i in range(n)]
         else:   # one GEMM for all adapters' dA: [G_0 | G_1 | ..]^T . x
             ga_sink = None
             if ACCUMULATE_ADAPTER_GRADS_IN_PLACE and all(a.grad is not None for a in pa):
@@ -229,28 +194,36 @@ class LoraGroupMatMul4Bit(torch.autograd.Function):
                 grad_as = [None] * n
             else:
                 ga_cat = torch.mm(g_cat.t(), xls[0])
+                r = lora_as[0].shape[0]
                 grad_as = [ga_cat[i * r:(i + 1) * r] for i in range(n)]
-        grad_bs = [_adapter_grad(pb[i], g2ds[i].t(), us[i]) for i in range(n)]
+        grad_bs = [_adapter_grad(pb[i], g2ds[i].t(), us[i]) if need_b[i] else None for i in range(n)]
         return (grad_x, None, None, None, *grad_xls, *([None] * n), *grad_as, *grad_bs)
 
 
+def lora_linear4bit(x: torch.Tensor, base, lora_a: torch.Tensor, lora_b: torch.Tensor, scaling: float,
+                    x_lora: torch.Tensor | None = None) -> torch.Tensor:
+    """`base(x) + (x_lora @ lora_a.T @ lora_b.T) * scaling` for a quantized `Linear4bit` base (no bias), fused.
+
+    `x_lora` is the LoRA branch's input when it differs from `x` (peft applies dropout to it); None = `x`.
+    Falls back to the two-step form (still on the GPU kernels) when the fused kernel does not cover the case
+    (fp16 compute dtype, rank not a multiple of 8 or > 64, bias present, unsupported shape)."""
+    x_loras = None if x_lora is None else [x_lora]
+    if _group_fusable(x, [base], [lora_a], [lora_b], x_loras):
+        return _apply(LoraMatMul4Bit, x, [base], scaling, x_loras, [lora_a], [lora_b])[0]
+    result = base(x)
+    xl = x if x_lora is None else x_lora
+    upd = torch.nn.functional.linear(torch.nn.functional.linear(xl.to(lora_a.dtype), lora_a), lora_b) * scaling
+    return result + upd.to(result.dtype)
+
+
 def lora_linear4bit_group(x: torch.Tensor, bases, lora_as, lora_bs, scaling: float, x_loras=None):
-    """Fused `[base_p(x) + (x_lora_p @ A_p.T @ B_p.T) * scaling for p]` for 2-3 Linear4bit of one shape on one input.
+    """Fused `[base_p(x) + (x_lora_p @ A_p.T @ B_p.T) * scaling for p]` for 1-3 Linear4bit of one shape on one input.
 
     Falls back to per-linear `lora_linear4bit` calls when the group does not qualify (different shapes, bias, ...)."""
-    n = len(bases)
-    shapes = {tuple(b.weight.quant_state.shape) if getattr(b.weight, "quant_state", None) is not None else None for b in bases}
-    ranks = {a.shape[0] for a in lora_as}
-    nested = {b.weight.quant_state.nested for b in bases if getattr(b.weight, "quant_state", None) is not None}
-    ok = (2 <= n <= 3 and len(shapes) == 1 and None not in shapes and len(ranks) == 1 and len(nested) == 1
-          and all(_fusable(x, bases[i], lora_as[i], lora_bs[i]) for i in range(n))
-          and (x_loras is None or all(t is not None for t in x_loras)))
-    if not ok:
+    if not _group_fusable(x, bases, lora_as, lora_bs, x_loras):
         return tuple(lora_linear4bit(x, bases[i], lora_as[i], lora_bs[i], scaling, None if x_loras is None else x_loras[i])
-                     for i in range(n))
-    xl = [None] * n if x_loras is None else list(x_loras)
-    states = tuple(b.weight.quant_state for b in bases)
-    return LoraGroupMatMul4Bit.apply(x, float(scaling), states, n, *xl, *[b.weight.t() for b in bases], *lora_as, *lora_bs)
+                     for i in range(len(bases)))
+    return _apply(LoraMatMul4Bit, x, bases, scaling, x_loras, lora_as, lora_bs)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -281,34 +254,24 @@ class DoraMatMul4Bit(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, scaling: float, states, n: int, *tensors):
-        # tensors = x_lora[0..n) (None: no dropout), packed_t[0..n), lora_a[0..n), lora_b[0..n), magnitude[0..n)
-        x_loras, packeds = tensors[:n], list(tensors[n:2 * n])
-        lora_as, lora_bs, mags = tensors[2 * n:3 * n], tensors[3 * n:4 * n], tensors[4 * n:5 * n]
+        x_loras, packeds, lora_as, lora_bs, mags = _split(tensors, n, 5)
         states = list(states)
-        x2d = _as_bf16_2d(x)
-        r = lora_as[0].shape[0]
+        x2d = F.as_bf16_2d(x)
         split = x_loras[0] is not None
-        norms = F.dora_weight_norm(packeds, states, list(lora_as), list(lora_bs), scaling)
+        norms = F.dora_weight_norm(packeds, states, lora_as, lora_bs, scaling)
         cs = [m.detach().float() / nrm for m, nrm in zip(mags, norms)]
-        out_dtype = torch.float32 if x.dtype == torch.float32 else torch.bfloat16
+        out_dtype = F.out_dtype_for(x.dtype)
+        xls, us = _project_inputs(x2d, x_loras, lora_as, scaling)
         if not split:
-            a_cat = _adjacent_rows(lora_as) if n > 1 else lora_as[0]
-            if a_cat is None:
-                a_cat = torch.cat(list(lora_as), 0)
-            u_cat = _project(x2d, a_cat, scaling)
-            us = [u_cat[:, i * r:(i + 1) * r] for i in range(n)]
-            xls = [x2d] * n
             vs = [(b.float() * c[:, None]).to(torch.bfloat16) for b, c in zip(lora_bs, cs)]    # diag(c) B
             ys = F.nf4_linear_group(False, [x2d] * n, packeds, states, us=us, vs=vs, out_dtype=out_dtype, row_scales=cs)
             qs_saved = ys                                            # Q = y / c: dm = sum_t dy * y / (c n)
         else:
-            xls = [_as_bf16_2d(t) for t in x_loras]
-            us = [_project(xls[i], lora_as[i], scaling) for i in range(n)]
             qs_saved = F.nf4_linear_group(False, xls, packeds, states, us=us, vs=[b.contiguous() for b in lora_bs])
             ps = F.nf4_linear_group(False, [x2d - xl for xl in xls], packeds, states)
             ys = [torch.addcmul(p.float(), q.float(), c).to(out_dtype) for p, q, c in zip(ps, qs_saved, cs)]
-        ctx.save_for_backward(*(xls if split else [x2d]), *us, *packeds, *lora_as, *lora_bs, *norms, *cs, *qs_saved)
-        ctx.params = (tuple(lora_as), tuple(lora_bs), tuple(mags))
+        ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs, *norms, *cs, *qs_saved)
+        ctx.params = (lora_as, lora_bs, mags)
         ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, split
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if split else None
@@ -318,36 +281,31 @@ class DoraMatMul4Bit(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grad_ys):
         n, split, s = ctx.n, ctx.split, ctx.scaling
-        saved = list(ctx.saved_tensors)
-        nx = n if split else 1
-        xls = saved[:nx] if split else [saved[0]] * n
-        rest = saved[nx:]
-        us, packeds, lora_as, lora_bs, norms, cs, qs_saved = (rest[i * n:(i + 1) * n] for i in range(7))
-        g2ds = [_as_bf16_2d(g) for g in grad_ys]
-        r = lora_as[0].shape[0]
-        # G_p = s (dy_p * c_p) . B_p = s dy_p . (diag(c_p) B_p), written side by side for one dA GEMM
-        g_cat = torch.empty((g2ds[0].shape[0], n * r), dtype=torch.bfloat16, device=g2ds[0].device)
-        gs = [_scaled_mm(g2ds[i], (lora_bs[i].float() * cs[i][:, None]).to(torch.bfloat16), s, out=g_cat[:, i * r:(i + 1) * r])
-              for i in range(n)]
-        out_dtype = torch.float32 if ctx.x_dtype == torch.float32 else torch.bfloat16
+        xls, us, packeds, lora_as, lora_bs, norms, cs, qs_saved = _split(ctx.saved_tensors, n, 8)
+        need_xl = ctx.needs_input_grad[4:4 + n]
+        g2ds = [F.as_bf16_2d(g) for g in grad_ys]
+        # G_p = s (dy_p * c_p) . B_p = s dy_p . (diag(c_p) B_p)
+        g_cat, gs = _project_grads(g2ds, [(b.float() * c[:, None]).to(torch.bfloat16) for b, c in zip(lora_bs, cs)], s)
+        out_dtype = F.out_dtype_for(ctx.x_dtype)
         grad_x = None
         grad_xls = [None] * n
         if split:
             if ctx.needs_input_grad[0]:
-                grad_x = F.nf4_linear_group(True, g2ds, list(packeds), ctx.states, out_dtype=out_dtype).view(ctx.x_shape)
+                grad_x = F.nf4_linear_group(True, g2ds, packeds, ctx.states, out_dtype=out_dtype).view(ctx.x_shape)
             for i in range(n):
-                if ctx.needs_input_grad[4 + i]:
+                if need_xl[i]:
                     shape, dtype = ctx.xl_meta[i]
                     grad_xls[i] = F.nf4_linear_group(True, [g2ds[i]], [packeds[i]], [ctx.states[i]], us=[gs[i]],
                                                      vs=[lora_as[i].contiguous()], row_scales=[cs[i] - 1.0],
-                                                     out_dtype=torch.float32 if dtype == torch.float32 else torch.bfloat16).view(shape)
+                                                     out_dtype=F.out_dtype_for(dtype)).view(shape)
         elif ctx.needs_input_grad[0]:
-            grad_x = F.nf4_linear_group(True, g2ds, list(packeds), ctx.states, us=gs, vs=[a.contiguous() for a in lora_as],
-                                        out_dtype=out_dtype, row_scales=list(cs)).view(ctx.x_shape)
+            grad_x = F.nf4_linear_group(True, g2ds, packeds, ctx.states, us=gs, vs=[a.contiguous() for a in lora_as],
+                                        out_dtype=out_dtype, row_scales=cs).view(ctx.x_shape)
         pa, pb, pm = ctx.params
         if split or n == 1:
             grad_as = [_adapter_grad(pa[i], gs[i].t(), xls[i]) for i in range(n)]
         else:
+            r = lora_as[0].shape[0]
             ga_cat = torch.mm(g_cat.t(), xls[0])
             grad_as = [_accumulate_or_return(pa[i], ga_cat[i * r:(i + 1) * r]) for i in range(n)]
         grad_bs, grad_ms = [], []
@@ -359,8 +317,9 @@ class DoraMatMul4Bit(torch.autograd.Function):
         return (grad_x, None, None, None, *grad_xls, *([None] * n), *grad_as, *grad_bs, *grad_ms)
 
 
-def _dora_fusable(x, base, lora_a, lora_b, magnitude) -> bool:
-    return _fusable(x, base, lora_a, lora_b) and magnitude.dtype == lora_a.dtype and magnitude.shape == (base.out_features,)
+def _dora_fusable(x, bases, lora_as, lora_bs, magnitudes, x_loras) -> bool:
+    return (_group_fusable(x, bases, lora_as, lora_bs, x_loras)
+            and all(m.dtype == a.dtype and m.shape == (b.out_features,) for b, a, m in zip(bases, lora_as, magnitudes)))
 
 
 def dora_linear4bit_peft(x, base, lora_a, lora_b, magnitude, scaling: float, x_lora=None):
@@ -388,26 +347,16 @@ def dora_linear4bit(x: torch.Tensor, base, lora_a: torch.Tensor, lora_b: torch.T
     """DoRA over a quantized `Linear4bit` base (peft `use_dora=True`), fused: the magnitude `m` rescales the rows of W inside
     the NF4 kernels.  `x_lora` is the dropped input of the adapter branch (None: no dropout / eval).  Falls back to
     `dora_linear4bit_peft` where `lora_linear4bit` falls back (rank, bias, dtype, shape)."""
-    if _dora_fusable(x, base, lora_a, lora_b, magnitude):
-        return DoraMatMul4Bit.apply(x, float(scaling), (base.weight.quant_state,), 1, x_lora, base.weight.t(), lora_a, lora_b,
-                                    magnitude)[0]
+    x_loras = None if x_lora is None else [x_lora]
+    if _dora_fusable(x, [base], [lora_a], [lora_b], [magnitude], x_loras):
+        return _apply(DoraMatMul4Bit, x, [base], scaling, x_loras, [lora_a], [lora_b], [magnitude])[0]
     return dora_linear4bit_peft(x, base, lora_a, lora_b, magnitude, scaling, x_lora)
 
 
 def dora_linear4bit_group(x: torch.Tensor, bases, lora_as, lora_bs, magnitudes, scaling: float, x_loras=None):
-    """`dora_linear4bit` for 2-3 Linear4bit of one shape on one input (q/k/v, gate/up): one launch per direction for the
+    """`dora_linear4bit` for 1-3 Linear4bit of one shape on one input (q/k/v, gate/up): one launch per direction for the
     GEMMs, one launch for their weight norms.  Falls back to per-linear calls when the group does not qualify."""
-    n = len(bases)
-    shapes = {tuple(b.weight.quant_state.shape) if getattr(b.weight, "quant_state", None) is not None else None for b in bases}
-    ranks = {a.shape[0] for a in lora_as}
-    nested = {b.weight.quant_state.nested for b in bases if getattr(b.weight, "quant_state", None) is not None}
-    ok = (2 <= n <= 3 and len(shapes) == 1 and None not in shapes and len(ranks) == 1 and len(nested) == 1
-          and all(_dora_fusable(x, bases[i], lora_as[i], lora_bs[i], magnitudes[i]) for i in range(n))
-          and (x_loras is None or all(t is not None for t in x_loras)))
-    if not ok:
+    if not _dora_fusable(x, bases, lora_as, lora_bs, magnitudes, x_loras):
         return tuple(dora_linear4bit(x, bases[i], lora_as[i], lora_bs[i], magnitudes[i], scaling,
-                                     None if x_loras is None else x_loras[i]) for i in range(n))
-    xl = [None] * n if x_loras is None else list(x_loras)
-    states = tuple(b.weight.quant_state for b in bases)
-    return DoraMatMul4Bit.apply(x, float(scaling), states, n, *xl, *[b.weight.t() for b in bases], *lora_as, *lora_bs,
-                                *magnitudes)
+                                     None if x_loras is None else x_loras[i]) for i in range(len(bases)))
+    return _apply(DoraMatMul4Bit, x, bases, scaling, x_loras, lora_as, lora_bs, magnitudes)

@@ -185,7 +185,8 @@ def test_fused_lora_step_vs_oracle(q, c_oracle, m, n, k, r):
 
 
 def test_fused_lora_autograd_matches_unfused(q):
-    """LoraMatMul4Bit (fused) vs peft's two-step form built from the same kernels: outputs and all gradients."""
+    """`lora_linear4bit` (fused: LoraMatMul4Bit with one linear) vs peft's two-step form built from the same kernels: outputs
+    and all gradients."""
     torch.manual_seed(0)
     base = q.nn.Linear4bit(512, 768, bias=False, compute_dtype=torch.bfloat16, quant_type="nf4").cuda()
     A = (torch.randn(64, 512, device="cuda") * 0.05).to(torch.bfloat16).requires_grad_(True)
