@@ -5,7 +5,6 @@
 // load per lane, two chunks in flight), every token's partial dot products stay in registers, warps meet in shared memory, bf16 rounding once.
 // Programmatic dependent launch on both sides: the skinny kernel that consumes U prefetches its weights while this runs.
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 #include "qb200_internal.h"
 #include "sm90_ptx.cuh"
@@ -72,26 +71,8 @@ __global__ void __launch_bounds__(32 * kProjWarps) lora_project_kernel(const __n
 template <int MT>
 static int launch_project(const void* x, int64_t ld_x, const void* a, float scale, void* u, int64_t ld_u, int M, int K, int R,
                           cudaStream_t stream) {
-  static const bool pdl = [] {
-    const char* e = getenv("QB200_PDL");
-    return !(e && atoi(e) == 0);
-  }();
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(unsigned(R), 1, 1);
-  cfg.blockDim = dim3(32 * kProjWarps, 1, 1);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, lora_project_kernel<MT>, static_cast<const __nv_bfloat16*>(x), ld_x,
-                                           static_cast<const __nv_bfloat16*>(a), scale, static_cast<__nv_bfloat16*>(u), ld_u, M, K);
-  if (e != cudaSuccess) {
-    (void)cudaGetLastError();
-    return set_error(int(e), "lora_project: cudaLaunchKernelEx failed");
-  }
-  return check_launch("lora_project");
+  return launch_pdl(lora_project_kernel<MT>, unsigned(R), 32 * kProjWarps, 0, stream, "lora_project", static_cast<const __nv_bfloat16*>(x),
+                    ld_x, static_cast<const __nv_bfloat16*>(a), scale, static_cast<__nv_bfloat16*>(u), ld_u, M, K);
 }
 
 }  // namespace qb200

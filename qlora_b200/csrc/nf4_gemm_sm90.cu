@@ -66,11 +66,6 @@ static int make_map_2d(CUtensorMap* m, CUtensorMapDataType dt, const void* base,
   return 0;
 }
 
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-
 // Largest token count served by the warp-level skinny kernel (nf4_gemv.cu) instead of the tensor-core wgmma kernel.
 static int skinny_max_m() {
   static int v = env_int("QB200_SKINNY_MAX_M", 16);
@@ -80,20 +75,6 @@ static int skinny_max_m() {
 static int debug_flags() {
   static int v = env_int("QB200_DEBUG_FLAGS", 0);
   return v;
-}
-
-// Programmatic dependent launch of the wgmma kernel (QB200_PDL=0 disables it: A/B timing).
-static bool use_pdl() {
-  static int v = env_int("QB200_PDL", 1);
-  return v != 0;
-}
-
-constexpr int kMaxDevices = 16;
-
-static int current_device() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
-  return dev;
 }
 
 // SMs of the CURRENT device (the library may serve several GPUs from one process: device_map='auto' in qlora.py); one
@@ -360,41 +341,13 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
     attr_set[dev][nested] = true;
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(unsigned(n_ctas), 1, 1);
-  cfg.blockDim = dim3(kNumThreads, 1, 1);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = use_pdl() ? 1 : 0;
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, maps, p, sched);
-  if (e != cudaSuccess) {
-    (void)cudaGetLastError();
-    return set_error(int(e), kTrans ? "nf4_linear_bwd_dx: cudaLaunchKernelEx failed" : "nf4_linear_fwd: cudaLaunchKernelEx failed");
-  }
-  int rc = check_launch(kTrans ? "nf4_linear_bwd_dx" : "nf4_linear_fwd");
+  const int rc = launch_pdl(kern, unsigned(n_ctas), kNumThreads, kSmemBytes, stream, kTrans ? "nf4_linear_bwd_dx" : "nf4_linear_fwd",
+                            maps, p, sched);
   if (rc || ksplit == 1) return rc;
   const int64_t TF = int64_t(T) * F;
   const int64_t nthreads = TF / 4;
-  cudaLaunchConfig_t rcfg{};
-  rcfg.gridDim = dim3(unsigned((nthreads + 255) / 256), 1, 1);
-  rcfg.blockDim = dim3(256, 1, 1);
-  rcfg.stream = stream;
-  cudaLaunchAttribute rattr[1];
-  rattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  rattr[0].val.programmaticStreamSerializationAllowed = 1;
-  rcfg.attrs = rattr;
-  rcfg.numAttrs = use_pdl() ? 1 : 0;
-  const cudaError_t re = cudaLaunchKernelEx(&rcfg, splitk_reduce_kernel, static_cast<const float*>(g.workspace), p.pr[0].bias, p.pr[0].out,
-                                            p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
-  if (re != cudaSuccess) {
-    (void)cudaGetLastError();
-    return set_error(int(re), "splitk_reduce: cudaLaunchKernelEx failed");
-  }
-  return check_launch("splitk_reduce");
+  return launch_pdl(splitk_reduce_kernel, unsigned((nthreads + 255) / 256), 256, 0, stream, "splitk_reduce",
+                    static_cast<const float*>(g.workspace), p.pr[0].bias, p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
 }
 
 static int validate_shape(int64_t M, int64_t N, int64_t K) {
@@ -460,10 +413,7 @@ static int linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, c
   // A grouped forward (q/k/v, gate/up) is nprob launches of them, chained by programmatic dependent launch.
   if (!is_bwd && out_dtype == QB200_DTYPE_BF16 && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
     for (int i = 0; i < nprob; ++i) {
-      const qb200_nf4_problem& q = probs[i];
-      rc = launch_nf4_skinny(q.in, q.ld_in, q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_u8 ? nullptr : q.absmax_f32,
-                             q.bias, q.out, q.ld_out, int(M), int(N), int(K), q.U, q.ld_u, q.V, int(R),
-                             row_scales ? row_scales[i] : nullptr, s);
+      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), s);
       if (rc) return rc;
     }
     return 0;

@@ -20,7 +20,6 @@
 // weights and every global weight load is a full 32-byte sector.  A CTA = one 8-row tile with the contraction split over
 // its warps; partial sums meet in shared memory.
 #include <cuda_bf16.h>
-#include <stdlib.h>
 
 #include "nf4_common.cuh"
 #include "nf4_table.cuh"
@@ -269,50 +268,17 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
   }
 }
 
-// Launch with programmatic stream serialization (QB200_PDL=0 disables it, as for the wgmma kernel).
-template <typename Kern, typename... Args>
-static int launch_pdl(Kern kern, unsigned grid, unsigned block, int smem, cudaStream_t stream, const char* what, Args... args) {
-  static const bool pdl = [] {
-    const char* e = getenv("QB200_PDL");
-    return !(e && atoi(e) == 0);
-  }();
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid, 1, 1);
-  cfg.blockDim = dim3(block, 1, 1);
-  cfg.dynamicSmemBytes = size_t(smem);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
-  if (e != cudaSuccess) {
-    (void)cudaGetLastError();
-    return set_error(int(e), what);
-  }
-  return check_launch(what);
-}
-
+// q's row pitches are resolved (non-zero).  Both instantiations take the full set of state pointers: the nested one reads
+// only absmax_u8 / code256 / absmax2 / offset, the plain one only absmax_f32.
 template <int NT, int kWarps, int kRing>
-static int launch_cfg(const void* x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256, const float* absmax2,
-                      const float* offset, const float* absmax_f32, const void* bias, void* y, int M, int N, int K, const void* U,
-                      int ld_u, const void* V, int R, int64_t ld_x, int64_t ld_y, const float* row_scale, cudaStream_t stream) {
-  const unsigned grid = unsigned(N / kRows);
+static int launch_cfg(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
   constexpr int smem = kWarps * NT * 8 * kSlabRowBytes + 256 * int(sizeof(float));
   static_assert(smem <= 48 * 1024, "static opt-in not needed below 48 KB");
-  const auto* xb = static_cast<const __nv_bfloat16*>(x);
-  const auto* bb = static_cast<const __nv_bfloat16*>(bias);
-  auto* yb = static_cast<__nv_bfloat16*>(y);
-  const uint8_t* no_u8 = nullptr;
-  const float* no_f = nullptr;
-  const auto* ub = static_cast<const __nv_bfloat16*>(U);
-  const auto* vb = static_cast<const __nv_bfloat16*>(V);
-  if (absmax_u8 != nullptr)
-    return launch_pdl(nf4_skinny_kernel<NT, kWarps, kRing, true>, grid, 32 * kWarps, smem, stream, "nf4_skinny", xb, packed, absmax_u8,
-                      code256, absmax2, offset, no_f, bb, yb, M, N, K, ub, ld_u, vb, R, ld_x, ld_y, row_scale);
-  return launch_pdl(nf4_skinny_kernel<NT, kWarps, kRing, false>, grid, 32 * kWarps, smem, stream, "nf4_skinny", xb, packed, no_u8, no_f,
-                    no_f, no_f, absmax_f32, bb, yb, M, N, K, ub, ld_u, vb, R, ld_x, ld_y, row_scale);
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel<NT, kWarps, kRing, true> : nf4_skinny_kernel<NT, kWarps, kRing, false>;
+  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny", static_cast<const __nv_bfloat16*>(q.in),
+                    q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const __nv_bfloat16*>(q.bias),
+                    static_cast<__nv_bfloat16*>(q.out), M, N, K, static_cast<const __nv_bfloat16*>(q.U), int(q.ld_u),
+                    static_cast<const __nv_bfloat16*>(q.V), R, q.ld_in, q.ld_out, row_scale);
 }
 
 template <int N>
@@ -477,59 +443,47 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
   }
 }
 
+// One token: row pitches do not matter.  State pointers as in launch_cfg.
 template <int kWarps, int kRing, int kBuf>
-static int launch_1tok(const void* x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256, const float* absmax2,
-                       const float* offset, const float* absmax_f32, const void* bias, void* y, int N, int K, const void* U,
-                       const void* V, int R, const float* row_scale, cudaStream_t stream) {
-  const unsigned grid = unsigned(N / kRows);
+static int launch_1tok(const qb200_nf4_problem& q, const float* row_scale, int N, int K, int R, cudaStream_t stream) {
   constexpr int kSlabs = kWarps * kBuf * kSlabRowBytes;
   constexpr int kRed = (kWarps + 1) * kRows * int(sizeof(float));
   constexpr int smem = (kSlabs > kRed ? kSlabs : kRed) + 256 * int(sizeof(float));
-  const auto* xb = static_cast<const __nv_bfloat16*>(x);
-  const auto* bb = static_cast<const __nv_bfloat16*>(bias);
-  auto* yb = static_cast<__nv_bfloat16*>(y);
-  const uint8_t* no_u8 = nullptr;
-  const float* no_f = nullptr;
-  if (absmax_u8 != nullptr)
-    return launch_pdl(nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, true>, grid, 32 * kWarps, smem, stream, "nf4_skinny_1tok", xb, packed,
-                      absmax_u8, code256, absmax2, offset, no_f, bb, yb, N, K, static_cast<const __nv_bfloat16*>(U),
-                      static_cast<const __nv_bfloat16*>(V), R, row_scale);
-  return launch_pdl(nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, false>, grid, 32 * kWarps, smem, stream, "nf4_skinny_1tok", xb, packed,
-                    no_u8, no_f, no_f, no_f, absmax_f32, bb, yb, N, K, static_cast<const __nv_bfloat16*>(U),
-                    static_cast<const __nv_bfloat16*>(V), R, row_scale);
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, true>
+                                           : nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, false>;
+  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny_1tok", static_cast<const __nv_bfloat16*>(q.in),
+                    q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const __nv_bfloat16*>(q.bias),
+                    static_cast<__nv_bfloat16*>(q.out), N, K, static_cast<const __nv_bfloat16*>(q.U),
+                    static_cast<const __nv_bfloat16*>(q.V), R, row_scale);
 }
 
 }  // namespace skinny
 
 // Internal: forward skinny GEMM, 16 tokens per launch (more tokens = more passes over the packed weights, which stay in L2);
-// optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; x / y / U may be column slices of wider row-major buffers (row
-// pitches ld_x / ld_y / ld_u in elements, 0 = dense); caller has validated pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0,
-// R <= 64, 16-byte aligned x / U rows and V).
-int launch_nf4_skinny(const void* x, int64_t ld_x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
-                      const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, void* y, int64_t ld_y,
-                      int M, int N, int K, const void* U, int64_t ld_u, const void* V, int R, const float* row_scale,
-                      cudaStream_t stream) {
+// optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U
+// may be column slices of wider row-major buffers (row pitches ld_in / ld_out / ld_u in elements, 0 = dense); caller has validated
+// pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0, R <= 64, 16-byte aligned in / U rows and V).
+int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
   if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");
-  if (R == 0) U = V = nullptr;
-  if (ld_u == 0) ld_u = R;
-  if (ld_x == 0) ld_x = K;
-  if (ld_y == 0) ld_y = N;
+  qb200_nf4_problem q = prob;   // advanced by one chunk of tokens per launch
+  if (R == 0) q.U = q.V = nullptr;
+  if (q.ld_u == 0) q.ld_u = R;
+  if (q.ld_in == 0) q.ld_in = K;
+  if (q.ld_out == 0) q.ld_out = N;
   constexpr int kChunk = 8 * skinny::kMaxNT;
   for (int m0 = 0; m0 < M; m0 += kChunk) {
     const int mc = M - m0 < kChunk ? M - m0 : kChunk;
-    const void* xc = static_cast<const __nv_bfloat16*>(x) + int64_t(m0) * ld_x;
-    const void* uc = U ? static_cast<const __nv_bfloat16*>(U) + int64_t(m0) * ld_u : nullptr;
-    void* yc = static_cast<__nv_bfloat16*>(y) + int64_t(m0) * ld_y;
     int rc;
-    if (mc == 1)   // one token: row pitches do not matter
-      rc = skinny::launch_1tok<4, 4, 2>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, N, K, uc, V, R, row_scale, stream);
+    if (mc == 1)
+      rc = skinny::launch_1tok<4, 4, 2>(q, row_scale, N, K, R, stream);
     else if (mc <= 8)
-      rc = skinny::launch_cfg<1, 4, 4>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, mc, N, K, uc, int(ld_u), V,
-                                       R, ld_x, ld_y, row_scale, stream);
+      rc = skinny::launch_cfg<1, 4, 4>(q, row_scale, mc, N, K, R, stream);
     else
-      rc = skinny::launch_cfg<2, 4, 4>(xc, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, yc, mc, N, K, uc, int(ld_u), V,
-                                       R, ld_x, ld_y, row_scale, stream);
+      rc = skinny::launch_cfg<2, 4, 4>(q, row_scale, mc, N, K, R, stream);
     if (rc) return rc;
+    q.in = static_cast<const __nv_bfloat16*>(q.in) + int64_t(kChunk) * q.ld_in;
+    if (q.U) q.U = static_cast<const __nv_bfloat16*>(q.U) + int64_t(kChunk) * q.ld_u;
+    q.out = static_cast<__nv_bfloat16*>(q.out) + int64_t(kChunk) * q.ld_out;
   }
   return 0;
 }

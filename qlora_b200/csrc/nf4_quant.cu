@@ -506,12 +506,8 @@ __global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __
 
 // QB200_DEQUANT_LUT=1 keeps the shared-memory-LUT kernels for every shape (A/B measurements, tests of that path)
 static bool dequant_lut_path() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("QB200_DEQUANT_LUT");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
+  static const bool v = env_int("QB200_DEQUANT_LUT", 0) == 1;
+  return v;
 }
 
 template <typename T>
@@ -519,6 +515,8 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
                                  const float* code256, const float* absmax2, const float* offset, int64_t n,
                                  int blocksize, int blocksize2, T* out, cudaStream_t stream) {
   if (n == 0) return 0;
+  // every kernel takes both forms' state pointers (those of the other form are null; blocksize2 = 1 for a plain state)
+  const bool nested = absmax_u8 != nullptr;
   const bool vec_ok = (reinterpret_cast<uintptr_t>(out) % 16 == 0) && (reinterpret_cast<uintptr_t>(packed) % 4 == 0);
   const int64_t nwords = (n + 7) / 8;
   const int threads = 256;
@@ -535,38 +533,24 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
         int64_t tb = (int64_t(nvec) + threads - 1) / threads;
         const int64_t tb_max = int64_t(device_sm_count()) * 4;   // persistent grid: 4 CTAs per SM
         if (tb > tb_max) tb = tb_max;
-        if (absmax_u8 != nullptr)
-          dequantize_nf4_tab_kernel<T, true><<<(unsigned)tb, threads, 0, stream>>>(
-              reinterpret_cast<const uint4*>(packed), nullptr, absmax_u8, code256, absmax2, offset, nvec, bs_shift - 2, bs2_shift,
-              reinterpret_cast<uint8_t*>(out));
-        else
-          dequantize_nf4_tab_kernel<T, false><<<(unsigned)tb, threads, 0, stream>>>(
-              reinterpret_cast<const uint4*>(packed), absmax, nullptr, nullptr, nullptr, nullptr, nvec, bs_shift - 2, 0,
-              reinterpret_cast<uint8_t*>(out));
+        const auto kern = nested ? dequantize_nf4_tab_kernel<T, true> : dequantize_nf4_tab_kernel<T, false>;
+        kern<<<(unsigned)tb, threads, 0, stream>>>(reinterpret_cast<const uint4*>(packed), absmax, absmax_u8, code256, absmax2, offset,
+                                                   nvec, bs_shift - 2, bs2_shift, reinterpret_cast<uint8_t*>(out));
         return check_launch("dequantize_nf4");
       }
       const int64_t fb_max = int64_t(device_sm_count()) * 16;
       const int64_t fb = blocks > fb_max ? fb_max : blocks;
-      if (absmax_u8 != nullptr)
-        dequantize_nf4_fast_kernel<T, true><<<(unsigned)fb, threads, 0, stream>>>(
-            reinterpret_cast<const uint32_t*>(packed), nullptr, absmax_u8, code256, absmax2, offset, uint32_t(nwords), bs_shift,
-            bs2_shift, reinterpret_cast<uint4*>(out));
-      else
-        dequantize_nf4_fast_kernel<T, false><<<(unsigned)fb, threads, 0, stream>>>(
-            reinterpret_cast<const uint32_t*>(packed), absmax, nullptr, nullptr, nullptr, nullptr, uint32_t(nwords), bs_shift, 0,
-            reinterpret_cast<uint4*>(out));
+      const auto kern = nested ? dequantize_nf4_fast_kernel<T, true> : dequantize_nf4_fast_kernel<T, false>;
+      kern<<<(unsigned)fb, threads, 0, stream>>>(reinterpret_cast<const uint32_t*>(packed), absmax, absmax_u8, code256, absmax2, offset,
+                                                 uint32_t(nwords), bs_shift, bs2_shift, reinterpret_cast<uint4*>(out));
       return check_launch("dequantize_nf4");
     }
   }
   const int64_t max_blocks = int64_t(device_sm_count()) * 8 * 8;  // grid-stride beyond a few waves of 8 resident CTAs/SM
   if (blocks > max_blocks) blocks = max_blocks;
-  if (absmax_u8 != nullptr) {
-    dequantize_nf4_kernel<T, true><<<(unsigned)blocks, threads, 0, stream>>>(packed, nullptr, absmax_u8, code256, absmax2,
-                                                                            offset, n, blocksize, blocksize2, vec_ok, out);
-  } else {
-    dequantize_nf4_kernel<T, false><<<(unsigned)blocks, threads, 0, stream>>>(packed, absmax, nullptr, nullptr, nullptr,
-                                                                             nullptr, n, blocksize, 1, vec_ok, out);
-  }
+  const auto kern = nested ? dequantize_nf4_kernel<T, true> : dequantize_nf4_kernel<T, false>;
+  kern<<<(unsigned)blocks, threads, 0, stream>>>(packed, absmax, absmax_u8, code256, absmax2, offset, n, blocksize, blocksize2, vec_ok,
+                                                 out);
   return check_launch("dequantize_nf4");
 }
 

@@ -1,7 +1,9 @@
-// Error reporting + version entry points of the C-ABI (include/qlora_b200.h).
+// Error reporting + version entry points of the C-ABI (include/qlora_b200.h), and the per-device and environment helpers
+// of qb200_internal.h.
 // Upstream bitsandbytes' CUDA_CHECK_RETURN prints and exit(1)s the process
 // (SURVEY.md 8b); here every entry point returns a status code instead.
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "qb200_internal.h"
@@ -22,16 +24,30 @@ int check_launch(const char* what) {
   return int(err);
 }
 
-int device_sm_count() {
-  constexpr int kMaxDevices = 16;
-  static int sms[kMaxDevices] = {0};
+int env_int(const char* name, int dflt) {
+  const char* e = getenv(name);
+  return e ? atoi(e) : dflt;
+}
+
+int current_device() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
+  return dev;
+}
+
+int device_sm_count() {
+  static int sms[kMaxDevices] = {0};
+  const int dev = current_device();
   if (sms[dev] == 0) {
     int n = 0;
     sms[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
   }
   return sms[dev];
+}
+
+bool use_pdl() {
+  static const bool v = env_int("QB200_PDL", 1) != 0;
+  return v;
 }
 }  // namespace qb200
 

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #include "../../include/qlora_b200.h"
 
@@ -10,12 +11,42 @@ namespace qb200 {
 int set_error(int code, const char* msg);
 // cudaPeekAtLastError() after a launch -> 0 or the cudaError_t (message recorded).
 int check_launch(const char* what);
-// Streaming multiprocessors of the calling thread's current device (cached per device); grid sizes are multiples of it.
+// Integer value of environment variable `name` (atoi), or `dflt` when it is unset.
+int env_int(const char* name, int dflt);
+// Per-device caches are indexed by current_device(): the calling thread's current device, 0 if it is unknown or >= kMaxDevices.
+constexpr int kMaxDevices = 16;
+int current_device();
+// Streaming multiprocessors of the current device (cached per device); grid sizes are multiples of it.
 int device_sm_count();
-// Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16, with an optional LoRA term U[M,R] . V[N,R]^T
-// and an optional per-row weight scale row_scale[N] (null: none); ld_* are row pitches in elements (0 = dense).
-int launch_nf4_skinny(const void* x, int64_t ld_x, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
-                      const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, void* y, int64_t ld_y,
-                      int M, int N, int K, const void* U, int64_t ld_u, const void* V, int R, const float* row_scale,
-                      cudaStream_t stream);
+// Programmatic dependent launch for every launch_pdl (QB200_PDL=0 disables it: A/B timing).
+bool use_pdl();
+
+// Launches kern<<<grid, block, smem, stream>>>(args...) with programmatic stream serialization when use_pdl(): the kernel
+// may start its prologue while the previous kernel of the stream still runs.  Returns 0 or the error (message recorded).
+template <typename... KArgs, typename... Args>
+int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, const char* what,
+               const Args&... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = use_pdl() ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, args...);
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();
+    char msg[160];
+    snprintf(msg, sizeof(msg), "%s: cudaLaunchKernelEx failed", what);
+    return set_error(int(e), msg);
+  }
+  return check_launch(what);
+}
+
+// Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16: problem q with its optional LoRA term
+// U[M,R] . V[N,R]^T (R = 0: none) and an optional per-row weight scale row_scale[N] (null: none).
+int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream);
 }  // namespace qb200
