@@ -169,12 +169,28 @@ int qb200_nf4_linear_group_scaled(int is_bwd, int nprob, const qb200_nf4_problem
                                   int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
                                   void* stream);
 
+/* ---- grouped form for either 16-bit compute type (fp16 compute: bnb_4bit_compute_dtype=torch.float16) ---------------
+ * qb200_nf4_linear_group_scaled with every 16-bit operand (in, bias, U, V and a 16-bit out) of type `dtype`:
+ *   QB200_DTYPE_BF16: the same launches as qb200_nf4_linear_group[_scaled];
+ *   QB200_DTYPE_F16 : the weights are fp16_rn(LUT[j]*absmax) -- dequantize_4bit's value for an fp16 or fp32 state, cast to
+ *                     fp16 -- and the result is rounded to fp16 once.
+ * out_dtype: `dtype`, or QB200_DTYPE_F32 = the dtype-rounded result widened.  row_scales may be NULL (no problem scaled).
+ * Forward calls with at most 16 tokens and a 16-bit output run the skinny kernels; the split-K workspace works as above.
+ * An unknown dtype, or an out_dtype that is neither `dtype` nor fp32, returns QB200_EINVAL. */
+int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales,
+                                 int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
+                                 void* stream);
+
 /* U[M,R] = scale * X[M,K] . A[R,K]^T for 1..16 tokens (bf16 in / out, fp32 sum, one rounding): the lora_A projection that
  * feeds qb200_nf4_linear_group's U operand during generation with an unmerged adapter — peft `lora.Linear.forward`'s
  * `lora_A(dropout(x))` (qlora.py:817-834 through PeftModel); replaces a split-K cuBLAS GEMM + reduce per projection.
  * ld_x / ld_u: row pitches in elements (0 = dense); x, A 16-byte aligned, K % 8 == 0.  Larger M: QB200_EUNSUPPORTED. */
 int qb200_lora_project(const void* x, int64_t ld_x, const void* A, float scale, void* U, int64_t ld_u, int64_t M, int64_t K,
                        int64_t R, void* stream);
+/* qb200_lora_project with x, A and U of type `dtype` (QB200_DTYPE_BF16: the same launch; QB200_DTYPE_F16: fp16 operands,
+ * fp32 sum, one fp16 rounding).  An unknown dtype returns QB200_EINVAL. */
+int qb200_lora_project_typed(int dtype, const void* x, int64_t ld_x, const void* A, float scale, void* U, int64_t ld_u, int64_t M,
+                             int64_t K, int64_t R, void* stream);
 
 /* ---- paged 32-bit AdamW (SURVEY.md 8f-3; qlora.py:198 optim='paged_adamw_32bit') ---------------------------
  * Replaces cadam32bit_grad_{fp32,fp16,bf16} (kernel kOptimizer32bit2State<T,ADAM>) and cget_managed_ptr / cprefetch.

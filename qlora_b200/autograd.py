@@ -7,10 +7,13 @@ qlora.py:249 via `bnb.nn.Linear4bit.forward`; SURVEY.md 8a rows a8, a11):
     backward: grad_A = grad_out @ dequantize_4bit(B, state).to(grad_out.dtype).t()   (B is weight.t())
               grad_B = None (frozen base weight: no dW GEMM), grad_bias = grad_out.sum(0)
 
-Here forward and dX run as ONE hand-written sm_90a kernel each (NF4 nibbles -> bf16 tiles in
-shared memory -> wgmma), so the dequantized W never reaches HBM.  Inputs the fused kernel
-does not cover (fp16/fp32 compute dtype, K % 64 != 0, ...) take the unfused *GPU* path
-(our dequant kernel + cuBLAS), which is also the "bnb-equivalent" baseline timed in bench.py.
+Here forward and dX run as ONE hand-written sm_90a kernel each (NF4 nibbles -> 16-bit tiles in
+shared memory -> wgmma), so the dequantized W never reaches HBM.  The fused compute dtypes are
+bf16 (over a bf16 quant state) and fp16 (over an fp16 or fp32 quant state: `qlora.py --fp16`,
+`bnb_4bit_compute_dtype=torch.float16`); for those, the kernels' weights fp16_rn / bf16_rn(LUT[j]*absmax) are exactly
+`dequantize_4bit(B, state).to(compute_dtype)`.  Inputs the fused kernel does not cover (fp32 compute dtype, a bf16 state
+under fp16 compute, K % 64 != 0, ...) take the unfused *GPU* path (our dequant kernel + cuBLAS), which is also the
+"bnb-equivalent" baseline timed in bench.py.
 """
 from __future__ import annotations
 
@@ -35,15 +38,16 @@ class MatMul4Bit(torch.autograd.Function):
     @staticmethod
     def forward(ctx, A, B, out=None, bias=None, quant_state: Optional[F.QuantState] = None, compute_dtype=None):
         # `compute_dtype` (extension): Linear4bit.forward's `x.to(compute_dtype)` ... `.to(inp_dtype)` folded into this node —
-        # fp32 activations are cast to bf16 once, and the kernel epilogue writes the bf16-rounded result widened to fp32
-        # (forward) / the fp32 input gradient (backward): the two output-side cast passes of a7 disappear.
+        # fp32 activations are cast to the 16-bit compute dtype (bf16 or fp16) once, and the kernel epilogue writes the
+        # rounded result widened to fp32 (forward) / the fp32 input gradient (backward): the two output-side cast passes of
+        # a7 disappear.
         ctx.io_dtype = None
         if compute_dtype is not None and A.dtype != compute_dtype:
-            if (A.dtype == torch.float32 and compute_dtype == torch.bfloat16 and USE_FUSED and out is None and prod(A.shape) > 0
-                    and B.shape[0] == 1 and F.fused_supported(quant_state, torch.bfloat16)):
+            if (A.dtype == torch.float32 and compute_dtype in (torch.bfloat16, torch.float16) and USE_FUSED and out is None
+                    and prod(A.shape) > 0 and B.shape[0] == 1 and F.fused_supported(quant_state, compute_dtype)):
                 ctx.io_dtype = torch.float32
             else:  # not coverable by the epilogue: behave exactly like the module-side casts
-                raise RuntimeError("MatMul4Bit: compute_dtype folding needs fp32 input + bf16 compute on the fused path")
+                raise RuntimeError("MatMul4Bit: compute_dtype folding needs fp32 input + bf16/fp16 compute on the fused path")
         ctx.is_empty = False
         if prod(A.shape) == 0:
             ctx.is_empty = True
@@ -56,9 +60,10 @@ class MatMul4Bit(torch.autograd.Function):
             return torch.empty(A.shape[:-1] + B_shape[:1], dtype=A.dtype, device=A.device)
 
         fused = ctx.io_dtype is not None or (USE_FUSED and B.shape[0] == 1 and F.fused_supported(quant_state, A.dtype))
+        cdt = compute_dtype if ctx.io_dtype is not None else A.dtype
         if fused:
-            b = bias if (bias is None or bias.dtype == torch.bfloat16) else bias.to(torch.bfloat16)
-            y = F.nf4_linear_fwd(F.as_bf16_2d(A), B, quant_state, b, out_dtype=F.out_dtype_for(A.dtype))
+            b = bias if (bias is None or bias.dtype == cdt) else bias.to(cdt)
+            y = F.nf4_linear_fwd(F.as_compute_2d(A, cdt), B, quant_state, b, out_dtype=F.out_dtype_for(A.dtype, cdt))
             output = y.view(*A.shape[:-1], quant_state.shape[0])
         else:
             output = torch.nn.functional.linear(A, _unfused_weight(B, quant_state, A.dtype).t(), bias)
@@ -67,7 +72,7 @@ class MatMul4Bit(torch.autograd.Function):
             output = out
 
         ctx.state = quant_state
-        ctx.fused = fused
+        ctx.fused, ctx.cdt = fused, cdt
         ctx.dtype_A, ctx.dtype_B, ctx.dtype_bias = A.dtype, B.dtype, None if bias is None else bias.dtype
         if any(ctx.needs_input_grad[:2]):
             ctx.tensors = (None, B)  # only the PACKED weight is kept for backward (no bf16 W is saved)
@@ -87,8 +92,9 @@ class MatMul4Bit(torch.autograd.Function):
             # sum over every leading dim (upstream sums dim 0 only, which is wrong for 3-D inputs)
             grad_bias = grad_output.reshape(-1, grad_output.shape[-1]).sum(0, dtype=ctx.dtype_bias)
         if req_gradA:
-            if ctx.fused and (ctx.io_dtype is not None or grad_output.dtype == torch.bfloat16):
-                dx = F.nf4_linear_bwd_dx(F.as_bf16_2d(grad_output), B, ctx.state, out_dtype=F.out_dtype_for(ctx.dtype_A))
+            if ctx.fused and (ctx.io_dtype is not None or grad_output.dtype == ctx.cdt):
+                dx = F.nf4_linear_bwd_dx(F.as_compute_2d(grad_output, ctx.cdt), B, ctx.state,
+                                         out_dtype=F.out_dtype_for(ctx.dtype_A, ctx.cdt))
                 grad_A = dx.view(*grad_output.shape[:-1], ctx.state.shape[1])
             else:
                 grad_A = torch.matmul(grad_output, _unfused_weight(B, ctx.state, grad_output.dtype).t())

@@ -2,10 +2,13 @@
 // generation (peft: lora_A(dropout(x)); qlora.py:817-834 with an unmerged PeftModel).  cuBLAS serves this 1 x 4096 x 64
 // product with a split-K GEMM + reduce (~10 us per projection in a decode chain, more than the NF4 GEMV it accompanies);
 // here it is one 256-thread CTA per adapter row: the eight warps split the contraction in 256-element chunks (one 16-byte
-// load per lane, two chunks in flight), every token's partial dot products stay in registers, warps meet in shared memory, bf16 rounding once.
+// load per lane, two chunks in flight), every token's partial dot products stay in registers, warps meet in shared memory,
+// one rounding to the operand type (bf16 or fp16).
 // Programmatic dependent launch on both sides: the skinny kernel that consumes U prefetches its weights while this runs.
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
+#include "nf4_table.cuh"
 #include "qb200_internal.h"
 #include "sm90_ptx.cuh"
 
@@ -13,28 +16,29 @@ namespace qb200 {
 
 constexpr int kProjWarps = 8;
 
-__device__ __forceinline__ float dot8_bf16(const uint4& a, const uint4& b) {
-  const __nv_bfloat162* a2 = reinterpret_cast<const __nv_bfloat162*>(&a);
-  const __nv_bfloat162* b2 = reinterpret_cast<const __nv_bfloat162*>(&b);
+template <typename T16>
+__device__ __forceinline__ float dot8(const uint4& a, const uint4& b) {
+  using T2 = typename Vec2<T16>::type;
+  const T2* a2 = reinterpret_cast<const T2*>(&a);
+  const T2* b2 = reinterpret_cast<const T2*>(&b);
   float acc = 0.0f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float2 fa = __bfloat1622float2(a2[i]), fb = __bfloat1622float2(b2[i]);
+    const float2 fa = widen2(a2[i]), fb = widen2(b2[i]);
     acc = fmaf(fa.x, fb.x, acc);
     acc = fmaf(fa.y, fb.y, acc);
   }
   return acc;
 }
 
-template <int MT>   // token slots kept in registers (1, 4, 8, 16); M <= MT
-__global__ void __launch_bounds__(32 * kProjWarps) lora_project_kernel(const __nv_bfloat16* __restrict__ x, int64_t ld_x,
-                                                                       const __nv_bfloat16* __restrict__ a, float scale,
-                                                                       __nv_bfloat16* __restrict__ u, int64_t ld_u, int M, int K) {
+template <typename T16, int MT>   // operand type (bf16, fp16); token slots kept in registers (1, 4, 8, 16); M <= MT
+__global__ void __launch_bounds__(32 * kProjWarps) lora_project_kernel(const T16* __restrict__ x, int64_t ld_x, const T16* __restrict__ a,
+                                                                       float scale, T16* __restrict__ u, int64_t ld_u, int M, int K) {
   __shared__ float s_part[kProjWarps][MT];
   const int j = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   ptx::grid_dep_launch();
   ptx::grid_dep_wait();                       // x is the previous kernel's output; the adapter may have just been updated
-  const __nv_bfloat16* arow = a + int64_t(j) * K;
+  const T16* arow = a + int64_t(j) * K;
   float acc[MT];
 #pragma unroll
   for (int m = 0; m < MT; ++m) acc[m] = 0.0f;
@@ -51,7 +55,7 @@ __global__ void __launch_bounds__(32 * kProjWarps) lora_project_kernel(const __n
       x1[m] = (m < M && two) ? *reinterpret_cast<const uint4*>(x + int64_t(m) * ld_x + k1) : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
-    for (int m = 0; m < MT; ++m) acc[m] += dot8_bf16(a0, x0[m]) + dot8_bf16(a1, x1[m]);
+    for (int m = 0; m < MT; ++m) acc[m] += dot8<T16>(a0, x0[m]) + dot8<T16>(a1, x1[m]);
   }
 #pragma unroll
   for (int m = 0; m < MT; ++m) {
@@ -64,23 +68,34 @@ __global__ void __launch_bounds__(32 * kProjWarps) lora_project_kernel(const __n
     float v = 0.0f;
 #pragma unroll
     for (int w = 0; w < kProjWarps; ++w) v += s_part[w][threadIdx.x];
-    u[int64_t(threadIdx.x) * ld_u + j] = __float2bfloat16_rn(v * scale);
+    u[int64_t(threadIdx.x) * ld_u + j] = round16<T16>(v * scale);
   }
 }
 
-template <int MT>
+template <typename T16, int MT>
 static int launch_project(const void* x, int64_t ld_x, const void* a, float scale, void* u, int64_t ld_u, int M, int K, int R,
                           cudaStream_t stream) {
-  return launch_pdl(lora_project_kernel<MT>, unsigned(R), 32 * kProjWarps, 0, stream, "lora_project", static_cast<const __nv_bfloat16*>(x),
-                    ld_x, static_cast<const __nv_bfloat16*>(a), scale, static_cast<__nv_bfloat16*>(u), ld_u, M, K);
+  return launch_pdl(lora_project_kernel<T16, MT>, unsigned(R), 32 * kProjWarps, 0, stream, "lora_project", static_cast<const T16*>(x),
+                    ld_x, static_cast<const T16*>(a), scale, static_cast<T16*>(u), ld_u, M, K);
+}
+
+template <typename T16>
+static int launch_project_m(const void* x, int64_t ld_x, const void* a, float scale, void* u, int64_t ld_u, int M, int K, int R,
+                            cudaStream_t s) {
+  if (M == 1) return launch_project<T16, 1>(x, ld_x, a, scale, u, ld_u, M, K, R, s);
+  if (M <= 4) return launch_project<T16, 4>(x, ld_x, a, scale, u, ld_u, M, K, R, s);
+  if (M <= 8) return launch_project<T16, 8>(x, ld_x, a, scale, u, ld_u, M, K, R, s);
+  return launch_project<T16, 16>(x, ld_x, a, scale, u, ld_u, M, K, R, s);
 }
 
 }  // namespace qb200
 
 using namespace qb200;
 
-extern "C" int qb200_lora_project(const void* x, int64_t ld_x, const void* a, float scale, void* u, int64_t ld_u, int64_t M,
-                                  int64_t K, int64_t R, void* stream) {
+extern "C" int qb200_lora_project_typed(int dtype, const void* x, int64_t ld_x, const void* a, float scale, void* u, int64_t ld_u,
+                                        int64_t M, int64_t K, int64_t R, void* stream) {
+  if (dtype != QB200_DTYPE_BF16 && dtype != QB200_DTYPE_F16)
+    return set_error(QB200_EINVAL, "lora_project_typed: dtype must be 2 (bf16) or 1 (fp16)");
   if (!x || !a || !u) return set_error(QB200_EINVAL, "lora_project: null pointer");
   if (M < 1 || M > 16) return set_error(QB200_EUNSUPPORTED, "lora_project: 1..16 tokens (larger batches are a library GEMM)");
   if (K < 8 || K % 8 != 0 || K > INT32_MAX || R < 1 || R > 65535) return set_error(QB200_EINVAL, "lora_project: bad shape");
@@ -90,8 +105,11 @@ extern "C" int qb200_lora_project(const void* x, int64_t ld_x, const void* a, fl
   if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(a) % 16)
     return set_error(QB200_EINVAL, "lora_project: x and A must be 16-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (M == 1) return launch_project<1>(x, ld_x, a, scale, u, ld_u, int(M), int(K), int(R), s);
-  if (M <= 4) return launch_project<4>(x, ld_x, a, scale, u, ld_u, int(M), int(K), int(R), s);
-  if (M <= 8) return launch_project<8>(x, ld_x, a, scale, u, ld_u, int(M), int(K), int(R), s);
-  return launch_project<16>(x, ld_x, a, scale, u, ld_u, int(M), int(K), int(R), s);
+  if (dtype == QB200_DTYPE_F16) return launch_project_m<__half>(x, ld_x, a, scale, u, ld_u, int(M), int(K), int(R), s);
+  return launch_project_m<__nv_bfloat16>(x, ld_x, a, scale, u, ld_u, int(M), int(K), int(R), s);
+}
+
+extern "C" int qb200_lora_project(const void* x, int64_t ld_x, const void* a, float scale, void* u, int64_t ld_u, int64_t M,
+                                  int64_t K, int64_t R, void* stream) {
+  return qb200_lora_project_typed(QB200_DTYPE_BF16, x, ld_x, a, scale, u, ld_u, M, K, R, stream);
 }

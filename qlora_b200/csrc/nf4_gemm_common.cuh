@@ -1,9 +1,10 @@
 // Shared pieces of the fused NF4 dequant + wgmma GEMM kernel (sm_90a): launch parameters, the register-resident
-// product-table dequant (16 x bf16_rne(LUT[j]*absmax) per NF4 block, nibbles resolved with PRMT byte permutes), the
+// product-table dequant (16 x T16_rne(LUT[j]*absmax) per NF4 block, T16 = bf16 or fp16; nibbles resolved with PRMT byte permutes), the
 // nested-absmax prefetch helper and the wgmma shared-memory descriptors.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -16,7 +17,7 @@ namespace qb200 {
 namespace gemm {
 
 constexpr int kBlockF = 128;   // features per work unit (two wgmma M=64 halves)
-constexpr int kBlockC = 64;    // contraction per step (one NF4 block; 128 B of bf16 = one swizzle row)
+constexpr int kBlockC = 64;    // contraction per step (one NF4 block; 128 B of 16-bit values = one swizzle row)
 constexpr int kMmaK = 16;
 constexpr int kATileBytes = kBlockF * kBlockC * 2;    // 16 KB: one dequantized wgmma A-operand tile
 constexpr int kWTileBytes = kBlockF * kBlockC / 2;    // 4 KB: the packed nibbles of that tile
@@ -32,10 +33,10 @@ struct Prob {
   const float* absmax2;
   const float* offset;
   const float* absmax_f32;   // non-nested state (or null)
-  const __nv_bfloat16* bias; // [F] or null (forward only)
+  const void* bias;          // [F] of the operand type (bf16 / fp16), or null (forward only)
   const float* row_scale;    // [N] or null: the absmax of every NF4 block of row n of W is multiplied by row_scale[n]
                              // (forward: Out = In . (diag(s) W)^T; dX: Out = In . diag(s) W).  Written by earlier kernels.
-  void* out;                 // [T, F] bf16 (or fp32 when Params::out_f32), row pitch ld_out elements
+  void* out;                 // [T, F] of the operand type (or fp32 when Params::out_f32), row pitch ld_out elements
   int64_t ld_out;
 };
 
@@ -47,7 +48,7 @@ struct Params {
   int T, F, C;
   int K;                     // row pitch of W[N,K] in elements
   int N;                     // rows of W
-  int lora_r;                // > 0: one extra bf16 contraction step per problem  Out += U_p[T,r] . V_p^T
+  int lora_r;                // > 0: one extra 16-bit contraction step per problem  Out += U_p[T,r] . V_p^T
   int out_f32;               // 1: the drain writes fp32 (Linear4bit called with fp32 activations: no separate cast pass)
   float* ws;                 // split-K: fp32 partial sums [ksplit, T, F] (null otherwise)
   int debug;                 // ablation flags for performance triage (QB200_DEBUG_FLAGS; 0 in production):

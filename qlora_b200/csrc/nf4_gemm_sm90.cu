@@ -94,8 +94,9 @@ static int num_ctas() {
   return ctas[dev];
 }
 
-// Split-K reduce: out[t, f] = bf16( sum_s ws[s, t, f] + bias[f] ), 4 features per thread (float4 loads, 8 B stores).
-__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ ws, const __nv_bfloat16* __restrict__ bias,
+// Split-K reduce: out[t, f] = T16( sum_s ws[s, t, f] + bias[f] ), 4 features per thread (float4 loads, 8 B stores).
+template <typename T16>
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ ws, const T16* __restrict__ bias,
                                                             void* __restrict__ out, int64_t ld_out, int out_f32, int64_t TF, int F,
                                                             int ksplit) {
   // programmatic dependent launch: this grid is queued while the GEMM kernel that writes `ws` still runs (its launch
@@ -112,18 +113,23 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
   const int64_t t = i4 / F;
   const int f = int(i4 - t * F);
   if (bias != nullptr) {
-    acc.x += __bfloat162float(bias[f]); acc.y += __bfloat162float(bias[f + 1]);
-    acc.z += __bfloat162float(bias[f + 2]); acc.w += __bfloat162float(bias[f + 3]);
+    acc.x += widen(bias[f]); acc.y += widen(bias[f + 1]);
+    acc.z += widen(bias[f + 2]); acc.w += widen(bias[f + 3]);
   }
   uint2 o;
-  o.x = ptx::cvt_bf16x2(acc.x, acc.y);
-  o.y = ptx::cvt_bf16x2(acc.z, acc.w);
+  o.x = round16x2<T16>(acc.x, acc.y);
+  o.y = round16x2<T16>(acc.z, acc.w);
   if (!out_f32) {
-    *reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(out) + t * ld_out + f) = o;
-  } else {   // the bf16-rounded sum, widened (Linear4bit called with fp32 activations)
+    *reinterpret_cast<uint2*>(static_cast<T16*>(out) + t * ld_out + f) = o;
+  } else {   // the T16-rounded sum, widened (Linear4bit called with fp32 activations)
     float4 w;
-    w.x = __uint_as_float(o.x << 16); w.y = __uint_as_float(o.x & 0xFFFF0000u);
-    w.z = __uint_as_float(o.y << 16); w.w = __uint_as_float(o.y & 0xFFFF0000u);
+    if constexpr (std::is_same<T16, __half>::value) {
+      const float2 lo = widen2(*reinterpret_cast<const __half2*>(&o.x)), hi = widen2(*reinterpret_cast<const __half2*>(&o.y));
+      w = make_float4(lo.x, lo.y, hi.x, hi.y);
+    } else {
+      w.x = __uint_as_float(o.x << 16); w.y = __uint_as_float(o.x & 0xFFFF0000u);
+      w.z = __uint_as_float(o.y << 16); w.w = __uint_as_float(o.y & 0xFFFF0000u);
+    }
     *reinterpret_cast<float4*>(static_cast<float*>(out) + t * ld_out + f) = w;
   }
 }
@@ -248,6 +254,7 @@ struct GroupArgs {
   int R;
   int M, N, K;
   int out_f32;
+  int f16;                          // 1: every 16-bit operand is fp16, 0: bf16
   void* workspace;
   int64_t workspace_bytes;
   const float* const* row_scales;   // [nprob] or null; an entry may be null (that problem is unscaled)
@@ -257,6 +264,7 @@ template <bool kTrans>
 static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   const int T = g.M, F = kTrans ? g.K : g.N, C = kTrans ? g.N : g.K;
   const bool nested = g.pr[0].absmax_u8 != nullptr;
+  const CUtensorMapDataType dt = g.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   Maps maps;
   Params p{};
   p.nprob = g.nprob;
@@ -268,20 +276,20 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   for (int i = 0; i < g.nprob; ++i) {
     const qb200_nf4_problem& q = g.pr[i];
     const int64_t ld_in = q.ld_in > 0 ? q.ld_in : C;
-    int rc = make_map_2d(&maps.in[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, q.in, uint64_t(C), uint64_t(T), uint64_t(ld_in) * 2,
+    int rc = make_map_2d(&maps.in[i], dt, q.in, uint64_t(C), uint64_t(T), uint64_t(ld_in) * 2,
                          kBlockC, kUnitT, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     if (g.R > 0) {
       // U[T, r] is a K-major B operand like the activation; V is [F, r] (forward, K-major A operand) or [r, F] (dX, MN-major)
       const int64_t ld_u = q.ld_u > 0 ? q.ld_u : g.R;
-      rc = make_map_2d(&maps.u[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, q.U, uint64_t(g.R), uint64_t(T), uint64_t(ld_u) * 2, kBlockC,
+      rc = make_map_2d(&maps.u[i], dt, q.U, uint64_t(g.R), uint64_t(T), uint64_t(ld_u) * 2, kBlockC,
                        kUnitT, CU_TENSOR_MAP_SWIZZLE_128B);
       if (rc) return rc;
       if (!kTrans)
-        rc = make_map_2d(&maps.v[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, q.V, uint64_t(g.R), uint64_t(F), uint64_t(g.R) * 2, kBlockC,
+        rc = make_map_2d(&maps.v[i], dt, q.V, uint64_t(g.R), uint64_t(F), uint64_t(g.R) * 2, kBlockC,
                          kBlockF, CU_TENSOR_MAP_SWIZZLE_128B);
       else
-        rc = make_map_2d(&maps.v[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, q.V, uint64_t(F), uint64_t(g.R), uint64_t(F) * 2, kBlockC,
+        rc = make_map_2d(&maps.v[i], dt, q.V, uint64_t(F), uint64_t(g.R), uint64_t(F) * 2, kBlockC,
                          kBlockC, CU_TENSOR_MAP_SWIZZLE_128B);
       if (rc) return rc;
     } else {
@@ -295,7 +303,7 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     d.absmax2 = q.absmax2;
     d.offset = q.offset;
     d.absmax_f32 = q.absmax_u8 ? nullptr : q.absmax_f32;
-    d.bias = static_cast<const __nv_bfloat16*>(q.bias);
+    d.bias = q.bias;
     d.row_scale = g.row_scales ? g.row_scales[i] : nullptr;
     d.out = p.group_sum ? g.pr[0].out : q.out;
     d.ld_out = (p.group_sum ? g.pr[0].ld_out : q.ld_out) > 0 ? (p.group_sum ? g.pr[0].ld_out : q.ld_out) : F;
@@ -333,21 +341,26 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     n_ctas = plan.n_ctas;
     memcpy(sched.start, plan.start, sizeof(sched.start));
   }
-  auto kern = nested ? nf4_gemm_wgmma_kernel<kTrans, true> : nf4_gemm_wgmma_kernel<kTrans, false>;
-  static bool attr_set[kMaxDevices][2] = {};
+  auto kern = g.f16 ? (nested ? nf4_gemm_wgmma_kernel<__half, kTrans, true> : nf4_gemm_wgmma_kernel<__half, kTrans, false>)
+                    : (nested ? nf4_gemm_wgmma_kernel<__nv_bfloat16, kTrans, true> : nf4_gemm_wgmma_kernel<__nv_bfloat16, kTrans, false>);
+  static bool attr_set[kMaxDevices][2][2] = {};
   const int dev = current_device();
-  if (!attr_set[dev][nested]) {   // the dynamic-smem opt-in is per device
+  if (!attr_set[dev][g.f16][nested]) {   // the dynamic-smem opt-in is per device and instantiation
     const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-    attr_set[dev][nested] = true;
+    attr_set[dev][g.f16][nested] = true;
   }
   const int rc = launch_pdl(kern, unsigned(n_ctas), kNumThreads, kSmemBytes, stream, kTrans ? "nf4_linear_bwd_dx" : "nf4_linear_fwd",
                             maps, p, sched);
   if (rc || ksplit == 1) return rc;
   const int64_t TF = int64_t(T) * F;
   const int64_t nthreads = TF / 4;
-  return launch_pdl(splitk_reduce_kernel, unsigned((nthreads + 255) / 256), 256, 0, stream, "splitk_reduce",
-                    static_cast<const float*>(g.workspace), p.pr[0].bias, p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
+  const unsigned blocks = unsigned((nthreads + 255) / 256);
+  if (g.f16)
+    return launch_pdl(splitk_reduce_kernel<__half>, blocks, 256, 0, stream, "splitk_reduce", static_cast<const float*>(g.workspace),
+                      static_cast<const __half*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
+  return launch_pdl(splitk_reduce_kernel<__nv_bfloat16>, blocks, 256, 0, stream, "splitk_reduce", static_cast<const float*>(g.workspace),
+                    static_cast<const __nv_bfloat16*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
 }
 
 static int validate_shape(int64_t M, int64_t N, int64_t K) {
@@ -385,12 +398,16 @@ using namespace qb200;
 
 extern "C" int qb200_has_fused_gemm(void) { return 1; }
 
-// ---- general entry point: 1..3 problems of one shape in ONE launch, each with an optional row scale ------------------
-static int linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales, int64_t R, int64_t M,
-                        int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
+// ---- general entry point: 1..3 problems of one shape in ONE launch, each with an optional row scale; 16-bit operands of
+// type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16) ---------------------------------------------------------------------
+static int linear_group(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales, int64_t R,
+                        int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (dtype != QB200_DTYPE_BF16 && dtype != QB200_DTYPE_F16)
+    return set_error(QB200_EINVAL, "nf4_linear_group_typed: dtype must be 2 (bf16) or 1 (fp16)");
   if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
-  if (out_dtype != QB200_DTYPE_BF16 && out_dtype != QB200_DTYPE_F32)
-    return set_error(QB200_EINVAL, "nf4_linear_group: out_dtype must be 2 (bf16) or 0 (fp32)");
+  if (out_dtype != dtype && out_dtype != QB200_DTYPE_F32)
+    return set_error(QB200_EINVAL, dtype == QB200_DTYPE_BF16 ? "nf4_linear_group: out_dtype must be 2 (bf16) or 0 (fp32)"
+                                                             : "nf4_linear_group_typed: out_dtype must be 1 (fp16) or 0 (fp32)");
   int rc = gemm::validate_shape(M, N, K);
   if (rc) return rc;
   if (R != 0 && (R < 0 || R > 64 || R % 8 != 0))
@@ -404,16 +421,16 @@ static int linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, c
     if (row_scales && reinterpret_cast<uintptr_t>(row_scales[i]) % 4 != 0)
       return set_error(QB200_EINVAL, "nf4_linear_group_scaled: row scales must be 4-byte aligned fp32");
   }
-  gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), out_dtype == QB200_DTYPE_F32 ? 1 : 0, workspace, workspace_bytes,
-                    row_scales};
+  gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), out_dtype == QB200_DTYPE_F32 ? 1 : 0,
+                    dtype == QB200_DTYPE_F16 ? 1 : 0, workspace, workspace_bytes, row_scales};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // forward with at most 16 tokens: warp-level skinny kernels (nf4_gemv.cu), SURVEY.md 8f-2 — with LoRA operands too (the
   // reference generates with the adapters attached: base GEMV + peft's two small matmuls; here the U . V^T term is the
   // kernel's epilogue)
   // A grouped forward (q/k/v, gate/up) is nprob launches of them, chained by programmatic dependent launch.
-  if (!is_bwd && out_dtype == QB200_DTYPE_BF16 && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
+  if (!is_bwd && out_dtype == dtype && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
     for (int i = 0; i < nprob; ++i) {
-      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), s);
+      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), dtype, s);
       if (rc) return rc;
     }
     return 0;
@@ -423,14 +440,20 @@ static int linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, c
 
 extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M, int64_t N,
                                       int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
-  return linear_group(is_bwd, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  return linear_group(is_bwd, QB200_DTYPE_BF16, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
 }
 
 extern "C" int qb200_nf4_linear_group_scaled(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales,
                                              int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
                                              int64_t workspace_bytes, void* stream) {
   if (!row_scales) return set_error(QB200_EINVAL, "nf4_linear_group_scaled: null row-scale array (NULL entries mean unscaled)");
-  return linear_group(is_bwd, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  return linear_group(is_bwd, QB200_DTYPE_BF16, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+}
+
+extern "C" int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs,
+                                            const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
+  return linear_group(is_bwd, dtype, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
 }
 
 extern "C" int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t K, int is_bwd) {

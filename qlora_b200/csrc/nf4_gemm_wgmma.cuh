@@ -1,8 +1,9 @@
 // Persistent fused NF4 dequant + wgmma GEMM (the production kernel; DESIGN.md 4.1).
 //
 // One CTA per SM.  Work unit = 128 features (two wgmma M=64 halves, one per consumer warpgroup) x up to 128 tokens (wgmma
-// N = 16..128), 64-wide contraction steps.  Per step the CTA dequantizes its 128 feature rows once into a bf16 A tile in
+// N = 16..128), 64-wide contraction steps.  Per step the CTA dequantizes its 128 feature rows once into a T16 A tile in
 // shared memory and TMA-loads the 128-row activation block; both warpgroups' MMAs read them straight from shared memory.
+// T16, the operand type of a launch, is bf16 or fp16: the tile layouts, swizzle and descriptors are the same for both.
 //
 // Schedule (host: nf4_gemm_sm90.cu).  The output of a launch is a strip of `n_fb x T` token-rows (n_fb = 128-feature blocks
 // of all problems of the launch, T = tokens); CTA c owns the CONTIGUOUS range [start[c], start[c+1]) of that strip and
@@ -72,7 +73,7 @@ struct Work {
   int kb0;     // first NF4 contraction step
   int nkb;     // NF4 contraction steps per segment
   int nseg;    // contraction segments (contraction-sum groups: one per problem)
-  int lora;    // 1: a bf16 LoRA step follows the NF4 steps of every segment
+  int lora;    // 1: a 16-bit LoRA step follows the NF4 steps of every segment
   int split;   // split-K index (0 when the unit covers the whole contraction)
 };
 
@@ -132,7 +133,7 @@ constexpr int kFirstDequantWarp = kConsumerWarps;
 constexpr int kNumThreads = 32 * (kFirstDequantWarp + kNumGroups * kGroupWarps);   // 640
 
 // Consumer warpgroup `wg`: all steps of one unit with wgmma N = kN (>= the unit's tokens), then the output stores.
-template <int kN, bool kTrans>
+template <typename T16, int kN, bool kTrans>
 __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, const Sched& sched, int wg, int warp, int lane,
                                              uint32_t smem_base, uint32_t aux, uint32_t& g, float (&acc)[ptx::kWgmmaMaxAcc]) {
   auto in_tile = [&](int s) { return smem_base + uint32_t(s) * kInSlotBytes; };
@@ -156,7 +157,7 @@ __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, con
       for (int k = 0; k < kBlockC / kMmaK; ++k) {
         const uint64_t a_adv = kTrans ? uint64_t((k * 2 * 1024) >> 4) : uint64_t((k * kMmaK * 2) >> 4);
         const uint64_t b_adv = uint64_t((k * kMmaK * 2) >> 4);
-        ptx::wgmma_bf16<kN, kTrans ? 1 : 0>(acc, a_desc + a_adv, b_desc + b_adv, (kb | k) != 0 ? 1u : 0u);
+        ptx::wgmma<T16, kN, kTrans ? 1 : 0>(acc, a_desc + a_adv, b_desc + b_adv, (kb | k) != 0 ? 1u : 0u);
       }
       ptx::wgmma_commit();
     }
@@ -192,23 +193,24 @@ __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, con
         }
       continue;
     }
-    const float bias_v = pr.bias != nullptr ? __bfloat162float(pr.bias[f]) : 0.0f;
+    const T16* bias = static_cast<const T16*>(pr.bias);
+    const float bias_v = bias != nullptr ? widen(bias[f]) : 0.0f;
 #pragma unroll
     for (int j = 0; j < kN / 8; ++j)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int t = w.t0 + 8 * j + tl + e;
         if (t >= p.T || 8 * j + tl + e >= w.nt) continue;
-        const __nv_bfloat16 o = __float2bfloat16_rn(acc[4 * j + 2 * h + e] + bias_v);
+        const T16 o = round16<T16>(acc[4 * j + 2 * h + e] + bias_v);
         if (!p.out_f32)
-          static_cast<__nv_bfloat16*>(pr.out)[int64_t(t) * pr.ld_out + f] = o;
-        else   // the bf16 rounding of the reference's GEMM output first, then widened: one store pass, no cast kernel
-          static_cast<float*>(pr.out)[int64_t(t) * pr.ld_out + f] = __bfloat162float(o);
+          static_cast<T16*>(pr.out)[int64_t(t) * pr.ld_out + f] = o;
+        else   // the 16-bit rounding of the reference's GEMM output first, then widened: one store pass, no cast kernel
+          static_cast<float*>(pr.out)[int64_t(t) * pr.ld_out + f] = widen(o);
       }
   }
 }
 
-template <bool kTrans, bool kNested>
+template <typename T16, bool kTrans, bool kNested>
 __global__ void __launch_bounds__(kNumThreads, 1)
 nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p, const __grid_constant__ Sched sched) {
   extern __shared__ uint8_t smem_raw[];
@@ -376,7 +378,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
         float am = fetch.resolve(s_code + pi_cur * 256, offset, valid_cur);
         if (rs_ptr != nullptr) am = __fmul_rn(am, rs_cur);
         Nf4Table tab;
-        build_table(am, tab);
+        build_table<T16>(am, tab);
         const uint32_t words[8] = {raw0.x, raw0.y, raw0.z, raw0.w, raw1.x, raw1.y, raw1.z, raw1.w};
         ptx::mbar_wait(empty(sa), empty_ph);
         const uint32_t dst = a_tile(sa) + st_base;
@@ -392,7 +394,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(full_a(sa));
       } else {
-        // LoRA step: the A-operand tile is plain bf16 (V rows of this unit's 128 features x r), TMA'd straight into the A
+        // LoRA step: the A-operand tile is plain T16 (V rows of this unit's 128 features x r), TMA'd straight into the A
         // slot in the same canonical layout the dequantizers produce (K-major fwd / MN-major dX).
         const int lora_pi = p.group_sum ? seg : u.prob;
         ptx::mbar_wait(empty(sa), empty_ph);
@@ -436,14 +438,14 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       const Work w = decode_work(a, cur_end, num_ctas, sched, p, num_kb, has_lora);
       a = w.next;
       switch (w.nt >> 4) {
-        case 1: consume_unit<16, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 2: consume_unit<32, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 3: consume_unit<48, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 4: consume_unit<64, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 5: consume_unit<80, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 6: consume_unit<96, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 7: consume_unit<112, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        default: consume_unit<128, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 1: consume_unit<T16, 16, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 2: consume_unit<T16, 32, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 3: consume_unit<T16, 48, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 4: consume_unit<T16, 64, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 5: consume_unit<T16, 80, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 6: consume_unit<T16, 96, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 7: consume_unit<T16, 112, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        default: consume_unit<T16, 128, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
       }
     }
   }

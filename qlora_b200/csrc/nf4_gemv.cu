@@ -6,10 +6,10 @@
 // README.md:135 calls 4-bit inference slow) and the few-token forward calls below the wgmma tile sizes.
 // The packed weight (N*K/2 B) + u8 absmax (N*K/64 B) are streamed exactly once; W is never materialised.
 //
-// Warp-level tensor-core path (mma.sync m16n8k16 bf16, fp32 accumulate) — the one place this library uses mma.sync:
+// Warp-level tensor-core path (mma.sync m16n8k16 bf16 or f16, fp32 accumulate) — the one place this library uses mma.sync:
 // the kernel is bound by the NF4 look-up on the ALU pipe (~3 PRMT/LOP/SHF per weight), not by tensor throughput, and
-// mma.sync takes its operands from registers: the look-up output (bf16x2 words holding the same bit-exact weights
-// bf16_rne(LUT[j] * absmax) as every other path) IS the B fragment, so nothing is unpacked, multiplied or staged per
+// mma.sync takes its operands from registers: the look-up output (16-bit pair words holding the same bit-exact weights
+// T16_rne(LUT[j] * absmax) as every other path; T16 = bf16 or fp16, the operand type of the launch) IS the B fragment, so nothing is unpacked, multiplied or staged per
 // weight, and 8 tokens cost the same as one.  (Round-1 history: a scalar-FMA GEMV paid look-up + unpack + FMA per weight
 // and token — ncu ALU pipe 61 %, DRAM 10 %, 12.1 us at 4096^2 for one token and 29.7 us for four.)
 //
@@ -20,6 +20,7 @@
 // weights and every global weight load is a full 32-byte sector.  A CTA = one 8-row tile with the contraction split over
 // its warps; partial sums meet in shared memory.
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include "nf4_common.cuh"
 #include "nf4_table.cuh"
@@ -32,7 +33,7 @@ namespace skinny {
 constexpr int kRows = 8;      // weight rows per CTA (MMA n)
 constexpr int kMaxNT = 2;     // up to 2 groups of 8 tokens per launch
 
-using Table = Nf4Table;   // nf4_table.cuh: 16 bf16 products of one NF4 block as low-byte / high-byte planes
+using Table = Nf4Table;   // nf4_table.cuh: 16 16-bit products of one NF4 block as low-byte / high-byte planes
 
 // (a & b) | c in one LOP3 with all three operands in registers (with immediates the compiler needs two)
 __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t b, uint32_t c) {
@@ -41,7 +42,7 @@ __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t b, uint32_t c) {
   return d;
 }
 
-// One packed word (8 nibbles, byte j = (element 2j << 4) | element 2j+1) -> 4 bf16x2 words in element order.
+// One packed word (8 nibbles, byte j = (element 2j << 4) | element 2j+1) -> 4 16-bit pair words in element order.
 // Per half (4 nibbles): PRMT picks entry (n & 7) from the first and the second 8 table entries, a third PRMT chooses
 // between them on bit 3 of the nibble; same for the high-byte plane; two more PRMTs interleave the planes.
 // prmt reads only bits [15:0] of its selector, so the selector words are prepared once for both halves.
@@ -58,18 +59,23 @@ __device__ __forceinline__ void lookup8(uint32_t word, const Table& t, uint32_t 
   }
 }
 
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                               uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+#define QB200_MMA_16816(ty)                                                                                               \
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32." ty "." ty ".f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};" \
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])                                                      \
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1))
+template <typename T16>
+__device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  if constexpr (std::is_same<T16, __half>::value) QB200_MMA_16816("f16");
+  else QB200_MMA_16816("bf16");
 }
+#undef QB200_MMA_16816
 
-// LoRA term of one output value: sum_j U[m, j] * V[row, j] over the rank (bf16 operands, fp32 sum) — the extra contraction
+// LoRA term of one output value: sum_j U[m, j] * V[row, j] over the rank (T16 operands, fp32 sum) — the extra contraction
 // step the wgmma kernel runs on the tensor core, here 8..64 multiply-adds in the epilogue.  U = scaling * x . A^T [M, r] comes
 // from the caller (one small GEMM), V = lora_B.weight [N, r]; rows are 16-byte aligned (r % 8 == 0).
-__device__ __forceinline__ float lora_dot(const __nv_bfloat16* __restrict__ u, const __nv_bfloat16* __restrict__ v, int r) {
+template <typename T16>
+__device__ __forceinline__ float lora_dot(const T16* __restrict__ u, const T16* __restrict__ v, int r) {
+  using T2 = typename Vec2<T16>::type;
   // all (at most 8 + 8) 16-byte loads are issued before the first multiply: one memory round trip, not r / 8 of them
   uint4 a[8], b[8];
 #pragma unroll
@@ -83,11 +89,11 @@ __device__ __forceinline__ float lora_dot(const __nv_bfloat16* __restrict__ u, c
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     if (8 * i < r) {
-      const __nv_bfloat162* a2 = reinterpret_cast<const __nv_bfloat162*>(&a[i]);
-      const __nv_bfloat162* b2 = reinterpret_cast<const __nv_bfloat162*>(&b[i]);
+      const T2* a2 = reinterpret_cast<const T2*>(&a[i]);
+      const T2* b2 = reinterpret_cast<const T2*>(&b[i]);
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float2 fa = __bfloat1622float2(a2[e]), fb = __bfloat1622float2(b2[e]);
+        const float2 fa = widen2(a2[e]), fb = widen2(b2[e]);
         acc = fmaf(fa.x, fb.x, acc);
         acc = fmaf(fa.y, fb.y, acc);
       }
@@ -132,12 +138,12 @@ constexpr int kSlabRowBytes = 512;       // x slab of one step: 4 blocks x 64 va
 //
 // B operand.  Each thread keeps kRing blocks (32 B of nibbles + absmax statistics each) in flight in registers
 // (the first version waited on one block at a time: ncu long-scoreboard 5.6 stalls / issue).
-template <int NT, int kWarps, int kRing, bool kNested>
+template <typename T16, int NT, int kWarps, int kRing, bool kNested>
 __global__ void __launch_bounds__(32 * kWarps, 4)
-nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
                   const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
-                  const float* __restrict__ absmax_f32, const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ y, int M,
-                  int N, int K, const __nv_bfloat16* __restrict__ lora_u, int ld_u, const __nv_bfloat16* __restrict__ lora_v,
+                  const float* __restrict__ absmax_f32, const T16* __restrict__ bias, T16* __restrict__ y, int M,
+                  int N, int K, const T16* __restrict__ lora_u, int ld_u, const T16* __restrict__ lora_v,
                   int lora_r, int64_t ld_x, int64_t ld_y, const float* __restrict__ row_scale) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   // [kWarps][NT * 8 tokens][512 B] x slabs, then 256 floats codebook; the slabs are re-used for the partial sums at the end
@@ -172,7 +178,7 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
   auto stage = [&](int bg) {
     const int blk = lane >> 3, j = lane & 7;
     const bool valid = bg + blk < nblk;
-    const __nv_bfloat16* src = x + (valid ? (int64_t(bg) << 6) + (lane << 3) : 0);
+    const T16* src = x + (valid ? (int64_t(bg) << 6) + (lane << 3) : 0);
     for (int tok = 0; tok < ntok; ++tok) {
       const uint32_t dst = slab + tok * kSlabRowBytes + blk * 128 + ((j ^ (blk | ((tok & 1) << 2))) << 4);
       cp_async_16(dst, src + int64_t(tok) * ld_x, valid);
@@ -227,17 +233,17 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
       if (row_scale != nullptr) am = __fmul_rn(am, rs);
       if (b >= nblk) am = 0.0f;
       Table tab;
-      build_table(am, tab);
+      build_table<T16>(am, tab);
       const uint32_t words[8] = {cur.lo.x, cur.lo.y, cur.lo.z, cur.lo.w, cur.hi.x, cur.hi.y, cur.hi.z, cur.hi.w};
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        uint32_t w[4];                                        // weights 8j..8j+7 of the block, bf16x2 in element order
+        uint32_t w[4];                                        // weights 8j..8j+7 of the block, 16-bit pairs in element order
         lookup8(words[j], tab, k4444, k3210, w);
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) {
           const uint4 v = lds128(frag + nt * 8 * kSlabRowBytes + ((j ^ swz) << 4));   // x[token, 64 b + 8 j .. + 8)
-          mma_bf16_16816(acc[nt][0], v.x, v.y, v.z, v.w, w[0], w[2]);
-          mma_bf16_16816(acc[nt][1], v.x, v.y, v.z, v.w, w[1], w[3]);
+          mma_16816<T16>(acc[nt][0], v.x, v.y, v.z, v.w, w[0], w[2]);
+          mma_16816<T16>(acc[nt][1], v.x, v.y, v.z, v.w, w[1], w[3]);
         }
       }
       __syncwarp();                                           // every lane has read the slab: overwrite it
@@ -263,22 +269,21 @@ nf4_skinny_kernel(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict
 #pragma unroll
     for (int w = 0; w < kWarps; ++w) v += s_red[(w * NT + nt) * 8 * kRows + i];
     if (lora_r > 0) v += lora_dot(lora_u + int64_t(m) * ld_u, lora_v + int64_t(row) * lora_r, lora_r);
-    if (bias != nullptr) v += __bfloat162float(bias[row]);
-    y[int64_t(m) * ld_y + row] = __float2bfloat16_rn(v);
+    if (bias != nullptr) v += widen(bias[row]);
+    y[int64_t(m) * ld_y + row] = round16<T16>(v);
   }
 }
 
 // q's row pitches are resolved (non-zero).  Both instantiations take the full set of state pointers: the nested one reads
 // only absmax_u8 / code256 / absmax2 / offset, the plain one only absmax_f32.
-template <int NT, int kWarps, int kRing>
+template <typename T16, int NT, int kWarps, int kRing>
 static int launch_cfg(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
   constexpr int smem = kWarps * NT * 8 * kSlabRowBytes + 256 * int(sizeof(float));
   static_assert(smem <= 48 * 1024, "static opt-in not needed below 48 KB");
-  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel<NT, kWarps, kRing, true> : nf4_skinny_kernel<NT, kWarps, kRing, false>;
-  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny", static_cast<const __nv_bfloat16*>(q.in),
-                    q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const __nv_bfloat16*>(q.bias),
-                    static_cast<__nv_bfloat16*>(q.out), M, N, K, static_cast<const __nv_bfloat16*>(q.U), int(q.ld_u),
-                    static_cast<const __nv_bfloat16*>(q.V), R, q.ld_in, q.ld_out, row_scale);
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel<T16, NT, kWarps, kRing, true> : nf4_skinny_kernel<T16, NT, kWarps, kRing, false>;
+  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny", static_cast<const T16*>(q.in), q.packed,
+                    q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias), static_cast<T16*>(q.out),
+                    M, N, K, static_cast<const T16*>(q.U), int(q.ld_u), static_cast<const T16*>(q.V), R, q.ld_in, q.ld_out, row_scale);
 }
 
 template <int N>
@@ -297,13 +302,14 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 // look-up costs 2.1 PRMT + 1.3 other ALU instructions per weight at 64 lanes/clk/SM (ncu, 4096x11008: ALU pipe 64 % of its
 // peak while SMs are active, issue slots 44 %, SMs active 71 % of the kernel) — a ceiling of ~2.7 TB/s of packed weights,
 // 0.42 of the HBM roofline, before launch and tail; DESIGN.md 4.3.
-template <int kWarps, int kRing, int kBuf, bool kNested>
+template <typename T16, int kWarps, int kRing, int kBuf, bool kNested>
 __global__ void __launch_bounds__(32 * kWarps, 4)
-nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
                        const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
-                       const float* __restrict__ absmax_f32, const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ y,
-                       int N, int K, const __nv_bfloat16* __restrict__ lora_u, const __nv_bfloat16* __restrict__ lora_v, int lora_r,
+                       const float* __restrict__ absmax_f32, const T16* __restrict__ bias, T16* __restrict__ y,
+                       int N, int K, const T16* __restrict__ lora_u, const T16* __restrict__ lora_v, int lora_r,
                        const float* __restrict__ row_scale) {
+  using T2 = typename Vec2<T16>::type;
   constexpr int kWarpSlab = kBuf * kSlabRowBytes;
   static_assert(kRing % kBuf == 0, "the slab of ring slot u is buffer u % kBuf");
   static_assert(32 * kWarps >= 16 * kRows, "the LoRA epilogue uses 16 lanes per weight row");
@@ -386,17 +392,17 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
       if (row_scale != nullptr) am = __fmul_rn(am, rs);
       if (4 * (warp + kWarps * s) + t >= nblk) am = 0.0f;
       Table tab;
-      build_table(am, tab);
+      build_table<T16>(am, tab);
       const int buf_off = (u % kBuf) * kSlabRowBytes;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const uint32_t word = j == 0 ? cur.lo.x : j == 1 ? cur.lo.y : j == 2 ? cur.lo.z : j == 3 ? cur.lo.w
                             : j == 4 ? cur.hi.x : j == 5 ? cur.hi.y : j == 6 ? cur.hi.z : cur.hi.w;
-        uint32_t w[4];                                        // weights 8j..8j+7 of the block, bf16x2 in element order
+        uint32_t w[4];                                        // weights 8j..8j+7 of the block, 16-bit pairs in element order
         lookup8(word, tab, k4444, k3210, w);
         const uint4 v = lds128(fword[j] + buf_off);           // x[64 b + 8 j .. + 8)
-        mma_bf16_16816(acc[0], v.x, v.y, v.z, v.w, w[0], w[2]);
-        mma_bf16_16816(acc[1], v.x, v.y, v.z, v.w, w[1], w[3]);
+        mma_16816<T16>(acc[0], v.x, v.y, v.z, v.w, w[0], w[2]);
+        mma_16816<T16>(acc[1], v.x, v.y, v.z, v.w, w[1], w[3]);
       }
       fetch(s + kRing, cur);                                  // clamped: a step beyond the row re-reads its last block
       __syncwarp();                                           // every lane has read the slab: overwrite it
@@ -421,10 +427,10 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
     if (row < kRows && c < lora_r) {
       const uint2 a = *reinterpret_cast<const uint2*>(lora_u + c);
       const uint2 b = __ldg(reinterpret_cast<const uint2*>(lora_v + int64_t(blockIdx.x * kRows + row) * lora_r + c));
-      const float2 a0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&a.x));
-      const float2 a1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&a.y));
-      const float2 b0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&b.x));
-      const float2 b1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&b.y));
+      const float2 a0 = widen2(*reinterpret_cast<const T2*>(&a.x));
+      const float2 a1 = widen2(*reinterpret_cast<const T2*>(&a.y));
+      const float2 b0 = widen2(*reinterpret_cast<const T2*>(&b.x));
+      const float2 b1 = widen2(*reinterpret_cast<const T2*>(&b.y));
       part = fmaf(a0.x, b0.x, fmaf(a0.y, b0.y, fmaf(a1.x, b1.x, a1.y * b1.y)));
     }
 #pragma unroll
@@ -438,54 +444,59 @@ nf4_skinny_kernel_1tok(const __nv_bfloat16* __restrict__ x, const uint8_t* __res
 #pragma unroll
     for (int w = 0; w < kWarps; ++w) v += s_red[w * kRows + threadIdx.x];
     if (lora_r > 0) v += s_red[kWarps * kRows + threadIdx.x];
-    if (bias != nullptr) v += __bfloat162float(bias[row]);
-    y[row] = __float2bfloat16_rn(v);
+    if (bias != nullptr) v += widen(bias[row]);
+    y[row] = round16<T16>(v);
   }
 }
 
 // One token: row pitches do not matter.  State pointers as in launch_cfg.
-template <int kWarps, int kRing, int kBuf>
+template <typename T16, int kWarps, int kRing, int kBuf>
 static int launch_1tok(const qb200_nf4_problem& q, const float* row_scale, int N, int K, int R, cudaStream_t stream) {
   constexpr int kSlabs = kWarps * kBuf * kSlabRowBytes;
   constexpr int kRed = (kWarps + 1) * kRows * int(sizeof(float));
   constexpr int smem = (kSlabs > kRed ? kSlabs : kRed) + 256 * int(sizeof(float));
-  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, true>
-                                           : nf4_skinny_kernel_1tok<kWarps, kRing, kBuf, false>;
-  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny_1tok", static_cast<const __nv_bfloat16*>(q.in),
-                    q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const __nv_bfloat16*>(q.bias),
-                    static_cast<__nv_bfloat16*>(q.out), N, K, static_cast<const __nv_bfloat16*>(q.U),
-                    static_cast<const __nv_bfloat16*>(q.V), R, row_scale);
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_1tok<T16, kWarps, kRing, kBuf, true>
+                                           : nf4_skinny_kernel_1tok<T16, kWarps, kRing, kBuf, false>;
+  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny_1tok", static_cast<const T16*>(q.in), q.packed,
+                    q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias), static_cast<T16*>(q.out),
+                    N, K, static_cast<const T16*>(q.U), static_cast<const T16*>(q.V), R, row_scale);
+}
+
+// 16 tokens per launch (more tokens = more passes over the packed weights, which stay in L2); q's row pitches are resolved.
+template <typename T16>
+static int launch_chunks(qb200_nf4_problem q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
+  constexpr int kChunk = 8 * kMaxNT;
+  for (int m0 = 0; m0 < M; m0 += kChunk) {
+    const int mc = M - m0 < kChunk ? M - m0 : kChunk;
+    int rc;
+    if (mc == 1)
+      rc = launch_1tok<T16, 4, 4, 2>(q, row_scale, N, K, R, stream);
+    else if (mc <= 8)
+      rc = launch_cfg<T16, 1, 4, 4>(q, row_scale, mc, N, K, R, stream);
+    else
+      rc = launch_cfg<T16, 2, 4, 4>(q, row_scale, mc, N, K, R, stream);
+    if (rc) return rc;
+    q.in = static_cast<const T16*>(q.in) + int64_t(kChunk) * q.ld_in;
+    if (q.U) q.U = static_cast<const T16*>(q.U) + int64_t(kChunk) * q.ld_u;
+    q.out = static_cast<T16*>(q.out) + int64_t(kChunk) * q.ld_out;
+  }
+  return 0;
 }
 
 }  // namespace skinny
 
-// Internal: forward skinny GEMM, 16 tokens per launch (more tokens = more passes over the packed weights, which stay in L2);
-// optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U
+// Internal: forward skinny GEMM, 16 tokens per launch, every 16-bit operand of type `dtype` (bf16 or fp16); optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U
 // may be column slices of wider row-major buffers (row pitches ld_in / ld_out / ld_u in elements, 0 = dense); caller has validated
 // pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0, R <= 64, 16-byte aligned in / U rows and V).
-int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
+int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, int dtype, cudaStream_t stream) {
   if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");
   qb200_nf4_problem q = prob;   // advanced by one chunk of tokens per launch
   if (R == 0) q.U = q.V = nullptr;
   if (q.ld_u == 0) q.ld_u = R;
   if (q.ld_in == 0) q.ld_in = K;
   if (q.ld_out == 0) q.ld_out = N;
-  constexpr int kChunk = 8 * skinny::kMaxNT;
-  for (int m0 = 0; m0 < M; m0 += kChunk) {
-    const int mc = M - m0 < kChunk ? M - m0 : kChunk;
-    int rc;
-    if (mc == 1)
-      rc = skinny::launch_1tok<4, 4, 2>(q, row_scale, N, K, R, stream);
-    else if (mc <= 8)
-      rc = skinny::launch_cfg<1, 4, 4>(q, row_scale, mc, N, K, R, stream);
-    else
-      rc = skinny::launch_cfg<2, 4, 4>(q, row_scale, mc, N, K, R, stream);
-    if (rc) return rc;
-    q.in = static_cast<const __nv_bfloat16*>(q.in) + int64_t(kChunk) * q.ld_in;
-    if (q.U) q.U = static_cast<const __nv_bfloat16*>(q.U) + int64_t(kChunk) * q.ld_u;
-    q.out = static_cast<__nv_bfloat16*>(q.out) + int64_t(kChunk) * q.ld_out;
-  }
-  return 0;
+  if (dtype == QB200_DTYPE_F16) return skinny::launch_chunks<__half>(q, row_scale, M, N, K, R, stream);
+  return skinny::launch_chunks<__nv_bfloat16>(q, row_scale, M, N, K, R, stream);
 }
 
 }  // namespace qb200

@@ -13,6 +13,31 @@
 
 namespace qb200 {
 
+// The 16-bit operand type T16 of the fused kernels (__nv_bfloat16 or __half): its two-element vector, round-to-nearest-even
+// from fp32 (one value, or two packed low | high) and the exact widening back to fp32.
+template <typename T16>
+struct Vec2 {
+  using type = __nv_bfloat162;
+};
+template <>
+struct Vec2<__half> {
+  using type = __half2;
+};
+template <typename T16>
+__device__ __forceinline__ T16 round16(float v) {
+  if constexpr (std::is_same<T16, __half>::value) return __float2half_rn(v);
+  else return __float2bfloat16_rn(v);
+}
+template <typename T16>
+__device__ __forceinline__ uint32_t round16x2(float lo, float hi) {
+  if constexpr (std::is_same<T16, __half>::value) return ptx::cvt_f16x2(lo, hi);
+  else return ptx::cvt_bf16x2(lo, hi);
+}
+__device__ __forceinline__ float widen(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
+__device__ __forceinline__ float2 widen2(__nv_bfloat162 v) { return __bfloat1622float2(v); }
+__device__ __forceinline__ float2 widen2(__half2 v) { return __half22float2(v); }
+
 struct Nf4Table {
   uint32_t tl[4], th[4];  // low / high byte planes of the 16 products
 };
@@ -23,9 +48,7 @@ __device__ __forceinline__ void build_table(float am, Nf4Table& t) {
   uint32_t p[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float lo = __fmul_rn(lut[2 * i], am), hi = __fmul_rn(lut[2 * i + 1], am);
-    if constexpr (std::is_same<T16, __half>::value) p[i] = ptx::cvt_f16x2(lo, hi);
-    else p[i] = ptx::cvt_bf16x2(lo, hi);
+    p[i] = round16x2<T16>(__fmul_rn(lut[2 * i], am), __fmul_rn(lut[2 * i + 1], am));
   }
 #pragma unroll
   for (int g = 0; g < 4; ++g) {

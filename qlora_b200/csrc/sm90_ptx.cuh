@@ -3,8 +3,11 @@
 // programmatic dependent launch.  Spellings follow the PTX ISA.
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace qb200 {
 namespace ptx {
@@ -84,7 +87,7 @@ __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.w
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // ---------------------------------------------------------------- wgmma ---------------
-// D[regs] (+)= A[smem desc] . B[smem desc], bf16 in, fp32 accumulate, one warpgroup (128 threads) per instruction.
+// D[regs] (+)= A[smem desc] . B[smem desc], bf16 or f16 in, fp32 accumulate, one warpgroup (128 threads) per instruction.
 // Accumulator fragment of m64nNk16 (thread t of the warpgroup, warp w = t / 32, lane l): d[4 j + 0, 1] = D[16 w + l / 4,
 // 8 j + 2 (l % 4) + {0, 1}], d[4 j + 2, 3] = the same columns of row 16 w + l / 4 + 8.
 constexpr int kWgmmaMaxAcc = 64;   // fp32 accumulators per thread of m64n128
@@ -98,82 +101,115 @@ __device__ __forceinline__ void wgmma_wait(float (&d)[kWgmmaMaxAcc]) {
   for (int i = 0; i < kWgmmaMaxAcc; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// generated: one wrapper per N = 16, 32, ..., 128 (the immediate shape); kTnspA = 1 for an MN-major A operand
-template <int kTnspA>
+// generated: one wrapper per N = 16, 32, ..., 128 (the immediate shape); kTnspA = 1 for an MN-major A operand.  The A and B
+// type is bf16 or f16 (T16 = __nv_bfloat16 / __half); both read the same shared-memory layouts and accumulate in fp32.
+#define QB200_WGMMA_M64N16(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n16(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N16("f16");
+  else QB200_WGMMA_M64N16("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N16
+#define QB200_WGMMA_M64N32(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n32(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N32("f16");
+  else QB200_WGMMA_M64N32("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N32
+#define QB200_WGMMA_M64N48(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n48(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N48("f16");
+  else QB200_WGMMA_M64N48("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N48
+#define QB200_WGMMA_M64N64(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n64(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N64("f16");
+  else QB200_WGMMA_M64N64("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N64
+#define QB200_WGMMA_M64N80(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, %43, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n80(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, %43, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N80("f16");
+  else QB200_WGMMA_M64N80("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N80
+#define QB200_WGMMA_M64N96(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n96(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N96("f16");
+  else QB200_WGMMA_M64N96("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N96
+#define QB200_WGMMA_M64N112(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n112k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, %59, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n112(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, %59, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N112("f16");
+  else QB200_WGMMA_M64N112("bf16");
 }
-template <int kTnspA>
+#undef QB200_WGMMA_M64N112
+#define QB200_WGMMA_M64N128(ty)                                                                                                      \
+  asm volatile(                                                                                                              \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                                 \
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." ty "." ty " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, 0;\n\t}" \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA))
+template <typename T16, int kTnspA>
 __device__ __forceinline__ void wgmma_m64n128(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(scale_d), "n"(kTnspA));
+  if constexpr (std::is_same<T16, __half>::value) QB200_WGMMA_M64N128("f16");
+  else QB200_WGMMA_M64N128("bf16");
 }
-template <int N, int kTnspA>
-__device__ __forceinline__ void wgmma_bf16(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
+#undef QB200_WGMMA_M64N128
+template <typename T16, int N, int kTnspA>
+__device__ __forceinline__ void wgmma(float (&d)[kWgmmaMaxAcc], uint64_t da, uint64_t db, uint32_t scale_d) {
   static_assert(N % 16 == 0 && N >= 16 && N <= 128, "m64nNk16 with N = 16..128");
-  if constexpr (N == 16) wgmma_m64n16<kTnspA>(d, da, db, scale_d);
-  else if constexpr (N == 32) wgmma_m64n32<kTnspA>(d, da, db, scale_d);
-  else if constexpr (N == 48) wgmma_m64n48<kTnspA>(d, da, db, scale_d);
-  else if constexpr (N == 64) wgmma_m64n64<kTnspA>(d, da, db, scale_d);
-  else if constexpr (N == 80) wgmma_m64n80<kTnspA>(d, da, db, scale_d);
-  else if constexpr (N == 96) wgmma_m64n96<kTnspA>(d, da, db, scale_d);
-  else if constexpr (N == 112) wgmma_m64n112<kTnspA>(d, da, db, scale_d);
-  else wgmma_m64n128<kTnspA>(d, da, db, scale_d);
+  if constexpr (N == 16) wgmma_m64n16<T16, kTnspA>(d, da, db, scale_d);
+  else if constexpr (N == 32) wgmma_m64n32<T16, kTnspA>(d, da, db, scale_d);
+  else if constexpr (N == 48) wgmma_m64n48<T16, kTnspA>(d, da, db, scale_d);
+  else if constexpr (N == 64) wgmma_m64n64<T16, kTnspA>(d, da, db, scale_d);
+  else if constexpr (N == 80) wgmma_m64n80<T16, kTnspA>(d, da, db, scale_d);
+  else if constexpr (N == 96) wgmma_m64n96<T16, kTnspA>(d, da, db, scale_d);
+  else if constexpr (N == 112) wgmma_m64n112<T16, kTnspA>(d, da, db, scale_d);
+  else wgmma_m64n128<T16, kTnspA>(d, da, db, scale_d);
 }
 
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {

@@ -422,11 +422,18 @@ def dequantize_nf4(A, quant_state=None, absmax=None, out=None, blocksize=64):
 # Fused linear entry points (new exports; SURVEY.md 8b "New export for the fused path")
 # --------------------------------------------------------------------------------------
 
+# Quant-state dtypes whose `dequantize_4bit(...).to(compute_dtype)` is exactly the fused kernels' product table
+# T16_rn(LUT[j] * absmax) for each fused compute dtype.  A bf16 state under fp16 compute rounds twice (bf16, then fp16) and
+# stays on the unfused path; so do fp16 / fp32 states under bf16 compute.
+_FUSED_STATE_DTYPES = {torch.bfloat16: (torch.bfloat16,), torch.float16: (torch.float16, torch.float32)}
+
+
 def fused_supported(quant_state: QuantState, compute_dtype: torch.dtype) -> bool:
     """Shapes/dtypes the fused wgmma kernel handles; everything else takes the unfused GPU path."""
-    if compute_dtype != torch.bfloat16 or quant_state.quant_type != "nf4" or quant_state.blocksize != 64:
+    if quant_state.quant_type != "nf4" or quant_state.blocksize != 64:
         return False
-    if quant_state.shape is None or len(quant_state.shape) != 2 or quant_state.dtype != torch.bfloat16:
+    if (quant_state.shape is None or len(quant_state.shape) != 2
+            or quant_state.dtype not in _FUSED_STATE_DTYPES.get(compute_dtype, ())):
         return False
     n_out, k_in = quant_state.shape
     if k_in % 64 != 0 or n_out % 8 != 0:
@@ -436,18 +443,19 @@ def fused_supported(quant_state: QuantState, compute_dtype: torch.dtype) -> bool
     return True
 
 
-def as_bf16_2d(t: Tensor) -> Tensor:
-    """`t` as the contiguous bf16 [rows, last dim] matrix the fused kernels read (cast and copied only where needed)."""
+def as_compute_2d(t: Tensor, dtype: torch.dtype = torch.bfloat16) -> Tensor:
+    """`t` as the contiguous [rows, last dim] matrix of the compute dtype (bf16 or fp16) the fused kernels read (cast and
+    copied only where needed)."""
     t2 = t.reshape(-1, t.shape[-1])
-    if t2.dtype != torch.bfloat16:
-        t2 = t2.to(torch.bfloat16)
+    if t2.dtype != dtype:
+        t2 = t2.to(dtype)
     return t2 if t2.is_contiguous() else t2.contiguous()
 
 
-def out_dtype_for(in_dtype: torch.dtype) -> torch.dtype:
-    """What a fused launch writes for activations of `in_dtype`: fp32 for fp32 (the kernel's epilogue widens the bf16-rounded
-    result, as `Linear4bit.forward` returns fp32 for fp32 input), else bf16."""
-    return torch.float32 if in_dtype == torch.float32 else torch.bfloat16
+def out_dtype_for(in_dtype: torch.dtype, compute_dtype: torch.dtype = torch.bfloat16) -> torch.dtype:
+    """What a fused launch writes for activations of `in_dtype`: fp32 for fp32 (the kernel's epilogue widens the result
+    rounded to the compute dtype, as `Linear4bit.forward` returns fp32 for fp32 input), else the compute dtype."""
+    return torch.float32 if in_dtype == torch.float32 else compute_dtype
 
 
 def _event_begin():
@@ -491,9 +499,16 @@ def _state_tensors(qs: QuantState, dev: torch.device):
     return None, None, None, None, qs.absmax
 
 
+_F16_CODE = DTYPE_CODE[torch.float16]
+
+
 def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None, vs=None, outs=None,
-                     out_dtype: torch.dtype = torch.bfloat16, row_scales=None):
+                     out_dtype: Optional[torch.dtype] = None, row_scales=None):
     """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group`).
+
+    The inputs' dtype (bf16 or fp16) is the compute dtype: U / V / bias are of it too and `out_dtype` is it (the default) or
+    fp32 (the result rounded to it, widened).  fp16 launches go through `qb200_nf4_linear_group_typed`; their event-log kinds
+    end in `_f16`.
 
     forward  (is_bwd=False): out_p = in_p . W_p^T (+bias_p) + U_p . V_p^T for every problem (the inputs may be one tensor);
                              returns the list of outputs.
@@ -513,16 +528,19 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     m = inputs[0].shape[0]
     r = 0 if us is None else us[0].shape[1]
     n_outs = 1 if is_bwd else n
+    cdt = inputs[0].dtype
+    assert cdt in (torch.bfloat16, torch.float16), f"inputs: bf16 or fp16, got {cdt}"
+    out_dtype = cdt if out_dtype is None else out_dtype
+    assert out_dtype in (cdt, torch.float32), f"out_dtype: {cdt} or fp32, got {out_dtype}"
     if outs is None:
-        dt = torch.float32 if out_dtype == torch.float32 else torch.bfloat16
-        outs = [torch.empty((m, f_out), dtype=dt, device=dev) for _ in range(n_outs)]
+        outs = [torch.empty((m, f_out), dtype=out_dtype, device=dev) for _ in range(n_outs)]
     if m == 0:
         return outs[0] if is_bwd else outs
     keep = []  # tensors that must outlive the launch call
     probs = (_lib.Nf4Problem * n)()
 
     def _rowmajor(t, cols, what):
-        assert t.dim() == 2 and t.shape == (m, cols) and t.dtype == torch.bfloat16, f"{what}: expected bf16 [{m}, {cols}]"
+        assert t.dim() == 2 and t.shape == (m, cols) and t.dtype == cdt, f"{what}: expected {cdt} [{m}, {cols}]"
         if t.stride(1) != 1 or (t.stride(0) % 8) or t.stride(0) < cols or (t.data_ptr() % 16):
             t = t.contiguous()
             keep.append(t)
@@ -546,20 +564,20 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
         b = None if biases is None else biases[i]
         if b is not None:
             assert not is_bwd and b.numel() == n_out
-            b = b.to(torch.bfloat16).contiguous()
+            b = b.to(cdt).contiguous()
             keep.append(b)
             pr.bias = b.data_ptr()
         if r:
             u = _rowmajor(us[i], r, "U")
             v = vs[i]
-            assert v.shape == ((r, k_in) if is_bwd else (n_out, r)) and v.dtype == torch.bfloat16
+            assert v.shape == ((r, k_in) if is_bwd else (n_out, r)) and v.dtype == cdt
             if not v.is_contiguous():
                 v = v.contiguous()
                 keep.append(v)
             pr.U, pr.ld_u, pr.V = u.data_ptr(), u.stride(0), v.data_ptr()
         if i < n_outs:
             o = outs[i]
-            assert o.shape == (m, f_out) and o.stride(1) == 1 and o.dtype == (torch.float32 if out_dtype == torch.float32 else torch.bfloat16)
+            assert o.shape == (m, f_out) and o.stride(1) == 1 and o.dtype == out_dtype
             pr.out, pr.ld_out = o.data_ptr(), o.stride(0)
     scales = None
     if row_scales is not None:
@@ -576,10 +594,14 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
     what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
-            + ("_scaled" if scales is not None else ""))
+            + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else ""))
     with torch.cuda.device(dev):
         ev = _event_begin()
-        if scales is None:
+        if cdt == torch.float16:
+            rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), _F16_CODE, n, ct.addressof(probs),
+                                                  None if scales is None else ct.addressof(scales), r, m, n_out, k_in,
+                                                  DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
+        elif scales is None:
             rc = lib.qb200_nf4_linear_group(int(is_bwd), n, ct.addressof(probs), r, m, n_out, k_in,
                                             0 if out_dtype == torch.float32 else 2, ptr(ws), ws_bytes, stream_ptr(dev))
         else:
@@ -591,7 +613,7 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
 
 
 def _linear_ex(is_bwd: bool, inp: Tensor, packed: Tensor, quant_state: QuantState, bias: Optional[Tensor] = None,
-               u: Optional[Tensor] = None, v: Optional[Tensor] = None, out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
+               u: Optional[Tensor] = None, v: Optional[Tensor] = None, out_dtype: Optional[torch.dtype] = None) -> Tensor:
     """One Linear4bit through the fused kernel (+ the split-K reduce when the schedule asks for a workspace)."""
     res = nf4_linear_group(is_bwd, [inp], [packed], [quant_state], None if bias is None else [bias],
                            None if u is None else [u], None if v is None else [v], out_dtype=out_dtype)
@@ -599,12 +621,13 @@ def _linear_ex(is_bwd: bool, inp: Tensor, packed: Tensor, quant_state: QuantStat
 
 
 def nf4_linear_fwd(x2d: Tensor, packed: Tensor, quant_state: QuantState, bias: Optional[Tensor] = None,
-                   out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
-    """Y[M,N] = X[M,K] . W^T (+bias) straight from the packed NF4 state (fused kernel)."""
+                   out_dtype: Optional[torch.dtype] = None) -> Tensor:
+    """Y[M,N] = X[M,K] . W^T (+bias) straight from the packed NF4 state (fused kernel); X bf16 or fp16, Y of X's dtype (or
+    `out_dtype` fp32)."""
     return _linear_ex(False, x2d, packed, quant_state, bias, out_dtype=out_dtype)
 
 
-def nf4_linear_bwd_dx(dy2d: Tensor, packed: Tensor, quant_state: QuantState, out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
+def nf4_linear_bwd_dx(dy2d: Tensor, packed: Tensor, quant_state: QuantState, out_dtype: Optional[torch.dtype] = None) -> Tensor:
     """dX[M,K] = dY[M,N] . W straight from the packed NF4 state (same kernel, W consumed MN-major)."""
     return _linear_ex(True, dy2d, packed, quant_state, out_dtype=out_dtype)
 
@@ -614,8 +637,8 @@ def lora_fused_supported(quant_state: QuantState, compute_dtype: torch.dtype, r:
 
 
 def nf4_linear_fwd_lora(x2d: Tensor, packed: Tensor, quant_state: QuantState, u: Tensor, v: Tensor,
-                        bias: Optional[Tensor] = None, out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
-    """Y[M,N] = X . W^T (+bias) + U . V^T in one launch (U[M,r] bf16, V[N,r] bf16 = lora_B.weight)."""
+                        bias: Optional[Tensor] = None, out_dtype: Optional[torch.dtype] = None) -> Tensor:
+    """Y[M,N] = X . W^T (+bias) + U . V^T in one launch (U[M,r], V[N,r] = lora_B.weight, of X's dtype)."""
     return _linear_ex(False, x2d, packed, quant_state, bias, u, v, out_dtype=out_dtype)
 
 
@@ -624,28 +647,34 @@ LORA_PROJECT_MAX_TOKENS = 16
 
 def lora_project(x2d: Tensor, lora_a: Tensor, scale: float) -> Tensor:
     """U[M,r] = scale * x2d . lora_a^T for at most 16 tokens (`qb200_lora_project`): the lora_A projection of a decode step.
-    bf16 operands, fp32 sum, one rounding — what `torch.addmm(..., alpha=scale)` returns, in one 3 us launch that chains
-    with the skinny kernel by programmatic dependent launch."""
+    bf16 (or fp16: `qb200_lora_project_typed`) operands of one dtype, fp32 sum, one rounding — what
+    `torch.addmm(..., alpha=scale)` returns, in one 3 us launch that chains with the skinny kernel by programmatic dependent
+    launch."""
     dev = _require_cuda(x2d, lora_a)
     m, k = x2d.shape
     r = lora_a.shape[0]
     assert 1 <= m <= LORA_PROJECT_MAX_TOKENS and lora_a.shape[1] == k
-    assert x2d.dtype == torch.bfloat16 and lora_a.dtype == torch.bfloat16
+    assert x2d.dtype in (torch.bfloat16, torch.float16) and lora_a.dtype == x2d.dtype
     if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k or x2d.data_ptr() % 16:
         x2d = x2d.contiguous()
     if not lora_a.is_contiguous() or lora_a.data_ptr() % 16:
         lora_a = lora_a.contiguous()
-    u = torch.empty((m, r), dtype=torch.bfloat16, device=dev)
+    u = torch.empty((m, r), dtype=x2d.dtype, device=dev)
     LAUNCH_COUNTER[0] += 1
+    lib = _lib.load()
     with torch.cuda.device(dev):
-        check(_lib.load().qb200_lora_project(ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u), r, m, k, r,
-                                            stream_ptr(dev)), "lora_project")
+        if x2d.dtype == torch.float16:
+            rc = lib.qb200_lora_project_typed(_F16_CODE, ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u), r, m, k, r,
+                                              stream_ptr(dev))
+        else:
+            rc = lib.qb200_lora_project(ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u), r, m, k, r, stream_ptr(dev))
+        check(rc, "lora_project")
     return u
 
 
 def nf4_linear_bwd_dx_lora(dy2d: Tensor, packed: Tensor, quant_state: QuantState, u: Tensor, vt: Tensor,
-                           out_dtype: torch.dtype = torch.bfloat16) -> Tensor:
-    """dX[M,K] = dY . W + U . Vt in one launch (U[M,r] bf16, Vt[r,K] bf16 = lora_A.weight)."""
+                           out_dtype: Optional[torch.dtype] = None) -> Tensor:
+    """dX[M,K] = dY . W + U . Vt in one launch (U[M,r], Vt[r,K] = lora_A.weight, of dY's dtype)."""
     return _linear_ex(True, dy2d, packed, quant_state, None, u, vt, out_dtype=out_dtype)
 
 

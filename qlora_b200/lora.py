@@ -6,14 +6,16 @@ peft's `lora.Linear4bit.forward` (reached from qlora.py:386-394 `get_peft_model`
     result = result + lora_B(lora_A(dropout(x))) * scaling
 
 i.e. two more GEMMs plus scale/add passes over [M, N] (and their mirror images in backward).  Here the low-rank
-update is ONE extra bf16 contraction step of the fused kernel, accumulated in the same register accumulators:
+update is ONE extra 16-bit contraction step of the fused kernel, accumulated in the same register accumulators:
 
     forward : Y  = X . W^T + U . B^T         U = scaling * (drop(X) . A^T)   [M, r]
     backward: dX = dY . W  + G . A           G = scaling * (dY . B)          [M, r]
               dA = G^T . drop(X)   dB = dY^T . U                             (the trainable adapters' grads)
 
-Only the skinny [M, r] projections stay separate (cuBLAS).  The sum is rounded to bf16 once (the unfused
-sequence rounds the base output and the update separately), so results agree with peft's to within one bf16 ulp.
+Only the skinny [M, r] projections stay separate (cuBLAS).  The sum is rounded to the compute dtype once (the unfused
+sequence rounds the base output and the update separately), so results agree with peft's to within one ulp of it.
+The compute dtype is bf16, or fp16 for a base with `compute_dtype=torch.float16` (over an fp16 or fp32 quant state); the
+adapters are of the compute dtype.
 
 Dropout (`--lora_dropout 0.1`, scripts/finetune_llama2_guanaco_7b.sh:42): the LoRA branch reads `x_lora = drop(x)`,
 passed as a second input.  Forward is unchanged (U comes from x_lora); in backward the LoRA term of the input gradient
@@ -27,8 +29,8 @@ separate accumulation of the input gradient — and the `x . A_p^T` projections 
 (`lora_linear4bit`) is the same call with one problem.
 
 fp32 activations (the reference casts its norms to fp32, qlora.py:400-401, so `Linear4bit.forward` sees fp32 in and
-returns fp32): the input is cast to bf16 once per call (once per GROUP for q/k/v) and the kernel's epilogue writes the
-bf16-rounded result widened to fp32 — the two output-side cast passes of `Linear4bit.forward` / its backward disappear.
+returns fp32): the input is cast to the compute dtype once per call (once per GROUP for q/k/v) and the kernel's epilogue
+writes the rounded result widened to fp32 — the two output-side cast passes of `Linear4bit.forward` / its backward disappear.
 """
 from __future__ import annotations
 
@@ -55,8 +57,8 @@ def _scaled_mm(a: torch.Tensor, b: torch.Tensor, scale: float, out: torch.Tensor
 def _project(x2d: torch.Tensor, lora_a: torch.Tensor, scale: float) -> torch.Tensor:
     """U = scale * x2d . lora_a^T.  A decode step (<= 16 tokens) takes the library's one-launch projection, which chains with
     the skinny kernel by programmatic dependent launch; everything else is one cuBLAS GEMM."""
-    if (x2d.shape[0] <= F.LORA_PROJECT_MAX_TOKENS and x2d.shape[1] % 8 == 0 and x2d.dtype == torch.bfloat16
-            and lora_a.dtype == torch.bfloat16 and lora_a.is_contiguous()):
+    if (x2d.shape[0] <= F.LORA_PROJECT_MAX_TOKENS and x2d.shape[1] % 8 == 0 and x2d.dtype in (torch.bfloat16, torch.float16)
+            and lora_a.dtype == x2d.dtype and lora_a.is_contiguous()):
         return F.lora_project(x2d, lora_a, scale)
     return _scaled_mm(x2d, lora_a.t(), scale)
 
@@ -102,11 +104,11 @@ def _apply(fn, x, bases, scaling: float, x_loras, *per_linear):
 
 
 def _project_inputs(x2d: torch.Tensor, x_loras, lora_as, scaling: float):
-    """(x_lora_p, U_p = scaling * x_lora_p . A_p^T) for every adapter, x_lora_p as bf16 [M, K].  Without dropout every x_lora_p
-    is x and ONE projection U_cat = scaling * x . [A_0; A_1; ..]^T is sliced into the U_p.  A single adapter is projected as it
+    """(x_lora_p, U_p = scaling * x_lora_p . A_p^T) for every adapter, x_lora_p as [M, K] of x2d's (the compute) dtype.
+    Without dropout every x_lora_p is x and ONE projection U_cat = scaling * x . [A_0; A_1; ..]^T is sliced into the U_p.  A single adapter is projected as it
     is: a cat of one non-contiguous A would be a contiguous copy, which moves a <= 16-token step onto the library's projection."""
     if x_loras[0] is not None:
-        xls = [F.as_bf16_2d(t) for t in x_loras]
+        xls = [F.as_compute_2d(t, x2d.dtype) for t in x_loras]
         return xls, [_project(xl, a, scaling) for xl, a in zip(xls, lora_as)]
     n, r = len(lora_as), lora_as[0].shape[0]
     a_cat = lora_as[0] if n == 1 else _adjacent_rows(lora_as)
@@ -120,15 +122,20 @@ def _project_grads(g2ds, vs, scaling: float):
     """G_p = scaling * dY_p . V_p ([M, r] each), written side by side into one [M, n r] buffer G_cat for a single dA GEMM;
     returns (G_cat, [G_p])."""
     r = vs[0].shape[1]
-    g_cat = torch.empty((g2ds[0].shape[0], len(vs) * r), dtype=torch.bfloat16, device=g2ds[0].device)
+    g_cat = torch.empty((g2ds[0].shape[0], len(vs) * r), dtype=g2ds[0].dtype, device=g2ds[0].device)
     return g_cat, [_scaled_mm(g, v, scaling, out=g_cat[:, i * r:(i + 1) * r]) for i, (g, v) in enumerate(zip(g2ds, vs))]
 
 
 def _fusable(x, base, lora_a, lora_b) -> bool:
+    """Whether one adapter-wrapped Linear4bit runs fused: the compute dtype is the base's fp16, else bf16 (a base with no or
+    bf16 compute dtype); x is of it or fp32, the adapters of it, and the fused kernel covers the quant state and the rank."""
     qs = getattr(base.weight, "quant_state", None)
-    return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float32) and base.bias is None and lora_a.dtype == torch.bfloat16
-            and lora_b.dtype == torch.bfloat16 and qs is not None and getattr(base, "compute_dtype", None) in (None, torch.bfloat16)
-            and F.lora_fused_supported(qs, torch.bfloat16, lora_a.shape[0]))
+    base_cdt = getattr(base, "compute_dtype", None)
+    if base_cdt not in (None, torch.bfloat16, torch.float16):
+        return False
+    cdt = torch.float16 if base_cdt == torch.float16 else torch.bfloat16
+    return (x.is_cuda and x.dtype in (cdt, torch.float32) and base.bias is None and lora_a.dtype == cdt and lora_b.dtype == cdt
+            and qs is not None and F.lora_fused_supported(qs, cdt, lora_a.shape[0]))
 
 
 def _group_fusable(x, bases, lora_as, lora_bs, x_loras) -> bool:
@@ -144,15 +151,17 @@ def _group_fusable(x, bases, lora_as, lora_bs, x_loras) -> bool:
 
 class LoraMatMul4Bit(torch.autograd.Function):
     """y_p = x . W_p^T + scaling * (x_lora_p . A_p^T) . B_p^T for n = 1..3 LoRA-wrapped Linear4bit of one shape applied to ONE
-    input (q/k/v, gate/up: one fused launch per direction).  x_lora_p = None for every p: no dropout, the adapters read x."""
+    input (q/k/v, gate/up: one fused launch per direction).  x_lora_p = None for every p: no dropout, the adapters read x.
+    The adapters' dtype (bf16 or fp16) is the compute dtype."""
 
     @staticmethod
     def forward(ctx, x, scaling: float, states, n: int, *tensors):
         x_loras, packeds, lora_as, lora_bs = _split(tensors, n, 4)
-        x2d = F.as_bf16_2d(x)
+        cdt = lora_as[0].dtype
+        x2d = F.as_compute_2d(x, cdt)
         xls, us = _project_inputs(x2d, x_loras, lora_as, scaling)
         ys = F.nf4_linear_group(False, [x2d] * n, packeds, list(states), us=us, vs=[b.contiguous() for b in lora_bs],
-                                out_dtype=F.out_dtype_for(x.dtype))
+                                out_dtype=F.out_dtype_for(x.dtype, cdt))
         ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs)
         ctx.adapters = (lora_as, lora_bs)   # the Parameter objects themselves (their .grad buffers, see _adapter_grad)
         ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, x_loras[0] is not None
@@ -166,9 +175,10 @@ class LoraMatMul4Bit(torch.autograd.Function):
         n, split = ctx.n, ctx.split
         xls, us, packeds, lora_as, lora_bs = _split(ctx.saved_tensors, n, 5)
         need_xl, _, need_a, need_b = _split(ctx.needs_input_grad[4:], n, 4)
-        g2ds = [F.as_bf16_2d(g) for g in grad_ys]
+        cdt = lora_as[0].dtype
+        g2ds = [F.as_compute_2d(g, cdt) for g in grad_ys]
         g_cat, gs = _project_grads(g2ds, lora_bs, ctx.scaling)
-        out_dtype = F.out_dtype_for(ctx.x_dtype)
+        out_dtype = F.out_dtype_for(ctx.x_dtype, cdt)
         grad_x = None
         grad_xls = [None] * n
         if split:
@@ -206,7 +216,7 @@ def lora_linear4bit(x: torch.Tensor, base, lora_a: torch.Tensor, lora_b: torch.T
 
     `x_lora` is the LoRA branch's input when it differs from `x` (peft applies dropout to it); None = `x`.
     Falls back to the two-step form (still on the GPU kernels) when the fused kernel does not cover the case
-    (fp16 compute dtype, rank not a multiple of 8 or > 64, bias present, unsupported shape)."""
+    (fp32 compute dtype, rank not a multiple of 8 or > 64, bias present, unsupported shape or quant-state dtype)."""
     x_loras = None if x_lora is None else [x_lora]
     if _group_fusable(x, [base], [lora_a], [lora_b], x_loras):
         return _apply(LoraMatMul4Bit, x, [base], scaling, x_loras, [lora_a], [lora_b])[0]
@@ -256,7 +266,7 @@ class DoraMatMul4Bit(torch.autograd.Function):
     def forward(ctx, x, scaling: float, states, n: int, *tensors):
         x_loras, packeds, lora_as, lora_bs, mags = _split(tensors, n, 5)
         states = list(states)
-        x2d = F.as_bf16_2d(x)
+        x2d = F.as_compute_2d(x)
         split = x_loras[0] is not None
         norms = F.dora_weight_norm(packeds, states, lora_as, lora_bs, scaling)
         cs = [m.detach().float() / nrm for m, nrm in zip(mags, norms)]
@@ -283,7 +293,7 @@ class DoraMatMul4Bit(torch.autograd.Function):
         n, split, s = ctx.n, ctx.split, ctx.scaling
         xls, us, packeds, lora_as, lora_bs, norms, cs, qs_saved = _split(ctx.saved_tensors, n, 8)
         need_xl = ctx.needs_input_grad[4:4 + n]
-        g2ds = [F.as_bf16_2d(g) for g in grad_ys]
+        g2ds = [F.as_compute_2d(g) for g in grad_ys]
         # G_p = s (dy_p * c_p) . B_p = s dy_p . (diag(c_p) B_p)
         g_cat, gs = _project_grads(g2ds, [(b.float() * c[:, None]).to(torch.bfloat16) for b, c in zip(lora_bs, cs)], s)
         out_dtype = F.out_dtype_for(ctx.x_dtype)
@@ -318,7 +328,8 @@ class DoraMatMul4Bit(torch.autograd.Function):
 
 
 def _dora_fusable(x, bases, lora_as, lora_bs, magnitudes, x_loras) -> bool:
-    return (_group_fusable(x, bases, lora_as, lora_bs, x_loras)
+    # bf16 compute only: fp16 DoRA takes the peft form
+    return (all(a.dtype == torch.bfloat16 for a in lora_as) and _group_fusable(x, bases, lora_as, lora_bs, x_loras)
             and all(m.dtype == a.dtype and m.shape == (b.out_features,) for b, a, m in zip(bases, lora_as, magnitudes)))
 
 
