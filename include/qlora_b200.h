@@ -181,6 +181,19 @@ int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_n
                                  int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
                                  void* stream);
 
+/* ---- grouped form with the quant state's dtype and an fp16 output under bf16 compute ---------------------------------
+ * qb200_nf4_linear_group_typed without row scales, for a quant state of `state_dtype` (the dtype `dequantize_4bit` returns
+ * for it).  The weights are exactly `dequantize_4bit(W, state).to(dtype)`:
+ *   dtype QB200_DTYPE_BF16: state bf16 or fp32 -> bf16_rn(LUT[j]*absmax);  state fp16 -> bf16_rn(fp16_rn(LUT[j]*absmax))
+ *                           (fp16 subnormals kept).  out_dtype bf16, fp32 (the bf16-rounded result widened) or fp16 (the
+ *                           bf16-rounded result rounded to fp16: `Linear4bit.forward`'s output cast for fp16 activations).
+ *   dtype QB200_DTYPE_F16 : state fp16 or fp32 -> fp16_rn(LUT[j]*absmax); out_dtype fp16 or fp32.
+ * Every other (dtype, state_dtype, out_dtype), including fp16 compute over a bf16 state, returns QB200_EINVAL before any
+ * launch.  Forward calls with at most 16 tokens and a 16-bit output run the skinny kernels; the split-K workspace works as
+ * above. */
+int qb200_nf4_linear_group_ex(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M,
+                              int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* U[M,R] = scale * X[M,K] . A[R,K]^T for 1..16 tokens (bf16 in / out, fp32 sum, one rounding): the lora_A projection that
  * feeds qb200_nf4_linear_group's U operand during generation with an unmerged adapter — peft `lora.Linear.forward`'s
  * `lora_A(dropout(x))` (qlora.py:817-834 through PeftModel); replaces a split-K cuBLAS GEMM + reduce per projection.

@@ -49,6 +49,7 @@ _SIGS = {
     "qb200_lora_project": ([_vp, _i64, _vp, ct.c_float, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
     "qb200_nf4_linear_group_typed": ([_i32, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, _vp], _i32),
     "qb200_lora_project_typed": ([_i32, _vp, _i64, _vp, ct.c_float, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
+    "qb200_nf4_linear_group_ex": ([_i32, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, _vp], _i32),
 }
 
 

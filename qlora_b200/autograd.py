@@ -9,10 +9,11 @@ qlora.py:249 via `bnb.nn.Linear4bit.forward`; SURVEY.md 8a rows a8, a11):
 
 Here forward and dX run as ONE hand-written sm_90a kernel each (NF4 nibbles -> 16-bit tiles in
 shared memory -> wgmma), so the dequantized W never reaches HBM.  The fused compute dtypes are
-bf16 (over a bf16 quant state) and fp16 (over an fp16 or fp32 quant state: `qlora.py --fp16`,
-`bnb_4bit_compute_dtype=torch.float16`); for those, the kernels' weights fp16_rn / bf16_rn(LUT[j]*absmax) are exactly
-`dequantize_4bit(B, state).to(compute_dtype)`.  Inputs the fused kernel does not cover (fp32 compute dtype, a bf16 state
-under fp16 compute, K % 64 != 0, ...) take the unfused *GPU* path (our dequant kernel + cuBLAS), which is also the
+bf16 (over a bf16, fp16 or fp32 quant state) and fp16 (over an fp16 or fp32 quant state: `qlora.py --fp16`,
+`bnb_4bit_compute_dtype=torch.float16`); for those, the kernels' weights are exactly
+`dequantize_4bit(B, state).to(compute_dtype)`: fp16_rn / bf16_rn(LUT[j]*absmax), and bf16_rn(fp16_rn(LUT[j]*absmax)) for an
+fp16 state under bf16 compute.  Inputs the fused kernel does not cover (fp32 compute dtype, a bf16 state under fp16
+compute, K % 64 != 0, ...) take the unfused *GPU* path (our dequant kernel + cuBLAS), which is also the
 "bnb-equivalent" baseline timed in bench.py.
 """
 from __future__ import annotations
@@ -38,16 +39,19 @@ class MatMul4Bit(torch.autograd.Function):
     @staticmethod
     def forward(ctx, A, B, out=None, bias=None, quant_state: Optional[F.QuantState] = None, compute_dtype=None):
         # `compute_dtype` (extension): Linear4bit.forward's `x.to(compute_dtype)` ... `.to(inp_dtype)` folded into this node —
-        # fp32 activations are cast to the 16-bit compute dtype (bf16 or fp16) once, and the kernel epilogue writes the
-        # rounded result widened to fp32 (forward) / the fp32 input gradient (backward): the two output-side cast passes of
-        # a7 disappear.
+        # fp32 activations (bf16 or fp16 compute) and fp16 activations (bf16 compute) are cast to the compute dtype once, and
+        # the kernel epilogue writes the rounded result in the input's dtype (forward) / the input gradient (backward): the
+        # two output-side cast passes of a7 disappear.
         ctx.io_dtype = None
         if compute_dtype is not None and A.dtype != compute_dtype:
-            if (A.dtype == torch.float32 and compute_dtype in (torch.bfloat16, torch.float16) and USE_FUSED and out is None
-                    and prod(A.shape) > 0 and B.shape[0] == 1 and F.fused_supported(quant_state, compute_dtype)):
-                ctx.io_dtype = torch.float32
+            foldable = ((A.dtype == torch.float32 and compute_dtype in (torch.bfloat16, torch.float16))
+                        or (A.dtype == torch.float16 and compute_dtype == torch.bfloat16))
+            if (foldable and USE_FUSED and out is None and prod(A.shape) > 0 and B.shape[0] == 1
+                    and F.fused_supported(quant_state, compute_dtype)):
+                ctx.io_dtype = A.dtype
             else:  # not coverable by the epilogue: behave exactly like the module-side casts
-                raise RuntimeError("MatMul4Bit: compute_dtype folding needs fp32 input + bf16/fp16 compute on the fused path")
+                raise RuntimeError("MatMul4Bit: compute_dtype folding needs fp32 input + bf16/fp16 compute or fp16 input + bf16 "
+                                   "compute, on the fused path")
         ctx.is_empty = False
         if prod(A.shape) == 0:
             ctx.is_empty = True

@@ -95,7 +95,8 @@ static int num_ctas() {
 }
 
 // Split-K reduce: out[t, f] = T16( sum_s ws[s, t, f] + bias[f] ), 4 features per thread (float4 loads, 8 B stores).
-template <typename T16>
+// kOutF16 (bf16 compute only): out is fp16, the bf16-rounded sum rounded again; out_f32 is not read.
+template <typename T16, bool kOutF16>
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ ws, const T16* __restrict__ bias,
                                                             void* __restrict__ out, int64_t ld_out, int out_f32, int64_t TF, int F,
                                                             int ksplit) {
@@ -119,7 +120,12 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
   uint2 o;
   o.x = round16x2<T16>(acc.x, acc.y);
   o.y = round16x2<T16>(acc.z, acc.w);
-  if (!out_f32) {
+  if constexpr (kOutF16) {   // the bf16 pairs widened exactly, then rounded to fp16
+    uint2 h;
+    h.x = ptx::cvt_f16x2(__uint_as_float(o.x << 16), __uint_as_float(o.x & 0xFFFF0000u));
+    h.y = ptx::cvt_f16x2(__uint_as_float(o.y << 16), __uint_as_float(o.y & 0xFFFF0000u));
+    *reinterpret_cast<uint2*>(static_cast<__half*>(out) + t * ld_out + f) = h;
+  } else if (!out_f32) {
     *reinterpret_cast<uint2*>(static_cast<T16*>(out) + t * ld_out + f) = o;
   } else {   // the T16-rounded sum, widened (Linear4bit called with fp32 activations)
     float4 w;
@@ -255,10 +261,17 @@ struct GroupArgs {
   int M, N, K;
   int out_f32;
   int f16;                          // 1: every 16-bit operand is fp16, 0: bf16
+  int state_f16;                    // bf16 compute over an fp16 quant state: weights bf16_rn(fp16_rn(LUT[j] * absmax))
+  int out_f16;                      // bf16 compute, fp16 output (the bf16-rounded result rounded to fp16); out_f32 is 0
   void* workspace;
   int64_t workspace_bytes;
   const float* const* row_scales;   // [nprob] or null; an entry may be null (that problem is unscaled)
 };
+
+template <typename T16, bool kTrans, bool kStateF16, bool kOutF16>
+static auto wgmma_kernel(bool nested) {
+  return nested ? nf4_gemm_wgmma_kernel<T16, kTrans, true, kStateF16, kOutF16> : nf4_gemm_wgmma_kernel<T16, kTrans, false, kStateF16, kOutF16>;
+}
 
 template <bool kTrans>
 static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
@@ -341,14 +354,16 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     n_ctas = plan.n_ctas;
     memcpy(sched.start, plan.start, sizeof(sched.start));
   }
-  auto kern = g.f16 ? (nested ? nf4_gemm_wgmma_kernel<__half, kTrans, true> : nf4_gemm_wgmma_kernel<__half, kTrans, false>)
-                    : (nested ? nf4_gemm_wgmma_kernel<__nv_bfloat16, kTrans, true> : nf4_gemm_wgmma_kernel<__nv_bfloat16, kTrans, false>);
-  static bool attr_set[kMaxDevices][2][2] = {};
-  const int dev = current_device();
-  if (!attr_set[dev][g.f16][nested]) {   // the dynamic-smem opt-in is per device and instantiation
+  using BF = __nv_bfloat16;
+  auto kern = g.f16         ? wgmma_kernel<__half, kTrans, false, false>(nested)
+              : g.state_f16 ? (g.out_f16 ? wgmma_kernel<BF, kTrans, true, true>(nested) : wgmma_kernel<BF, kTrans, true, false>(nested))
+                            : (g.out_f16 ? wgmma_kernel<BF, kTrans, false, true>(nested) : wgmma_kernel<BF, kTrans, false, false>(nested));
+  static bool attr_set[kMaxDevices][2][2][2][2] = {};
+  bool& attr_done = attr_set[current_device()][g.f16][g.state_f16][g.out_f16][nested];
+  if (!attr_done) {   // the dynamic-smem opt-in is per device and instantiation
     const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-    attr_set[dev][g.f16][nested] = true;
+    attr_done = true;
   }
   const int rc = launch_pdl(kern, unsigned(n_ctas), kNumThreads, kSmemBytes, stream, kTrans ? "nf4_linear_bwd_dx" : "nf4_linear_fwd",
                             maps, p, sched);
@@ -357,10 +372,11 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   const int64_t nthreads = TF / 4;
   const unsigned blocks = unsigned((nthreads + 255) / 256);
   if (g.f16)
-    return launch_pdl(splitk_reduce_kernel<__half>, blocks, 256, 0, stream, "splitk_reduce", static_cast<const float*>(g.workspace),
+    return launch_pdl(splitk_reduce_kernel<__half, false>, blocks, 256, 0, stream, "splitk_reduce", static_cast<const float*>(g.workspace),
                       static_cast<const __half*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
-  return launch_pdl(splitk_reduce_kernel<__nv_bfloat16>, blocks, 256, 0, stream, "splitk_reduce", static_cast<const float*>(g.workspace),
-                    static_cast<const __nv_bfloat16*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
+  return launch_pdl(g.out_f16 ? splitk_reduce_kernel<BF, true> : splitk_reduce_kernel<BF, false>, blocks, 256, 0, stream, "splitk_reduce",
+                    static_cast<const float*>(g.workspace), static_cast<const BF*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32,
+                    TF, F, ksplit);
 }
 
 static int validate_shape(int64_t M, int64_t N, int64_t K) {
@@ -399,15 +415,13 @@ using namespace qb200;
 extern "C" int qb200_has_fused_gemm(void) { return 1; }
 
 // ---- general entry point: 1..3 problems of one shape in ONE launch, each with an optional row scale; 16-bit operands of
-// type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16) ---------------------------------------------------------------------
-static int linear_group(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales, int64_t R,
-                        int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
-  if (dtype != QB200_DTYPE_BF16 && dtype != QB200_DTYPE_F16)
-    return set_error(QB200_EINVAL, "nf4_linear_group_typed: dtype must be 2 (bf16) or 1 (fp16)");
+// type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16) over a quant state of `state_dtype`, output of `out_dtype` -----------
+// The entry points validate the three dtypes; a bf16 launch reads the double-rounded table only for an fp16 state (a bf16
+// or fp32 state gives the table bf16_rn(LUT[j] * absmax)), and an fp16 launch's table is the same for every state it takes.
+static int linear_group(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs,
+                        const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
+                        int64_t workspace_bytes, void* stream) {
   if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
-  if (out_dtype != dtype && out_dtype != QB200_DTYPE_F32)
-    return set_error(QB200_EINVAL, dtype == QB200_DTYPE_BF16 ? "nf4_linear_group: out_dtype must be 2 (bf16) or 0 (fp32)"
-                                                             : "nf4_linear_group_typed: out_dtype must be 1 (fp16) or 0 (fp32)");
   int rc = gemm::validate_shape(M, N, K);
   if (rc) return rc;
   if (R != 0 && (R < 0 || R > 64 || R % 8 != 0))
@@ -421,16 +435,19 @@ static int linear_group(int is_bwd, int dtype, int nprob, const qb200_nf4_proble
     if (row_scales && reinterpret_cast<uintptr_t>(row_scales[i]) % 4 != 0)
       return set_error(QB200_EINVAL, "nf4_linear_group_scaled: row scales must be 4-byte aligned fp32");
   }
+  const bool bf16 = dtype == QB200_DTYPE_BF16;
   gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), out_dtype == QB200_DTYPE_F32 ? 1 : 0,
-                    dtype == QB200_DTYPE_F16 ? 1 : 0, workspace, workspace_bytes, row_scales};
+                    dtype == QB200_DTYPE_F16 ? 1 : 0, bf16 && state_dtype == QB200_DTYPE_F16 ? 1 : 0,
+                    bf16 && out_dtype == QB200_DTYPE_F16 ? 1 : 0, workspace, workspace_bytes, row_scales};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // forward with at most 16 tokens: warp-level skinny kernels (nf4_gemv.cu), SURVEY.md 8f-2 — with LoRA operands too (the
-  // reference generates with the adapters attached: base GEMV + peft's two small matmuls; here the U . V^T term is the
-  // kernel's epilogue)
+  // forward with at most 16 tokens and a 16-bit output: warp-level skinny kernels (nf4_gemv.cu), SURVEY.md 8f-2 — with LoRA
+  // operands too (the reference generates with the adapters attached: base GEMV + peft's two small matmuls; here the U . V^T
+  // term is the kernel's epilogue)
   // A grouped forward (q/k/v, gate/up) is nprob launches of them, chained by programmatic dependent launch.
-  if (!is_bwd && out_dtype == dtype && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
+  if (!is_bwd && out_dtype != QB200_DTYPE_F32 && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
     for (int i = 0; i < nprob; ++i) {
-      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), dtype, s);
+      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), dtype, g.state_f16,
+                             g.out_f16, s);
       if (rc) return rc;
     }
     return 0;
@@ -438,22 +455,55 @@ static int linear_group(int is_bwd, int dtype, int nprob, const qb200_nf4_proble
   return is_bwd ? gemm::launch_gemm<true>(g, s) : gemm::launch_gemm<false>(g, s);
 }
 
+// dtype / out_dtype rule of the bf16 and typed entry points: the operand dtype is bf16 or fp16, the output is of it or fp32
+static int check_typed_dtypes(int dtype, int out_dtype) {
+  if (dtype != QB200_DTYPE_BF16 && dtype != QB200_DTYPE_F16)
+    return set_error(QB200_EINVAL, "nf4_linear_group_typed: dtype must be 2 (bf16) or 1 (fp16)");
+  if (out_dtype != dtype && out_dtype != QB200_DTYPE_F32)
+    return set_error(QB200_EINVAL, dtype == QB200_DTYPE_BF16 ? "nf4_linear_group: out_dtype must be 2 (bf16) or 0 (fp32)"
+                                                             : "nf4_linear_group_typed: out_dtype must be 1 (fp16) or 0 (fp32)");
+  return 0;
+}
+
 extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M, int64_t N,
                                       int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
-  return linear_group(is_bwd, QB200_DTYPE_BF16, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  const int rc = check_typed_dtypes(QB200_DTYPE_BF16, out_dtype);
+  if (rc) return rc;
+  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace,
+                      workspace_bytes, stream);
 }
 
 extern "C" int qb200_nf4_linear_group_scaled(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales,
                                              int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
                                              int64_t workspace_bytes, void* stream) {
   if (!row_scales) return set_error(QB200_EINVAL, "nf4_linear_group_scaled: null row-scale array (NULL entries mean unscaled)");
-  return linear_group(is_bwd, QB200_DTYPE_BF16, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  const int rc = check_typed_dtypes(QB200_DTYPE_BF16, out_dtype);
+  if (rc) return rc;
+  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace,
+                      workspace_bytes, stream);
 }
 
 extern "C" int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs,
                                             const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype,
                                             void* workspace, int64_t workspace_bytes, void* stream) {
-  return linear_group(is_bwd, dtype, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  const int rc = check_typed_dtypes(dtype, out_dtype);
+  if (rc) return rc;
+  return linear_group(is_bwd, dtype, dtype, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+}
+
+extern "C" int qb200_nf4_linear_group_ex(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int64_t R,
+                                         int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
+                                         void* stream) {
+  const bool f32_or_f16_state = state_dtype == QB200_DTYPE_F32 || state_dtype == QB200_DTYPE_F16;
+  const bool ok = dtype == QB200_DTYPE_BF16
+                      ? (f32_or_f16_state || state_dtype == QB200_DTYPE_BF16) &&
+                            (out_dtype == QB200_DTYPE_BF16 || out_dtype == QB200_DTYPE_F32 || out_dtype == QB200_DTYPE_F16)
+                      : dtype == QB200_DTYPE_F16 && f32_or_f16_state && (out_dtype == QB200_DTYPE_F16 || out_dtype == QB200_DTYPE_F32);
+  if (!ok)
+    return set_error(QB200_EINVAL, "nf4_linear_group_ex: unsupported (dtype, state_dtype, out_dtype): bf16 compute takes a bf16, fp16 "
+                                   "or fp32 state and writes bf16, fp32 or fp16; fp16 compute takes an fp16 or fp32 state and "
+                                   "writes fp16 or fp32");
+  return linear_group(is_bwd, dtype, state_dtype, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
 }
 
 extern "C" int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t K, int is_bwd) {

@@ -4,6 +4,7 @@
 // N = 16..128), 64-wide contraction steps.  Per step the CTA dequantizes its 128 feature rows once into a T16 A tile in
 // shared memory and TMA-loads the 128-row activation block; both warpgroups' MMAs read them straight from shared memory.
 // T16, the operand type of a launch, is bf16 or fp16: the tile layouts, swizzle and descriptors are the same for both.
+// Under bf16 compute the quant state may be fp16 (kStateF16: double-rounded product table) and the output fp16 (kOutF16).
 //
 // Schedule (host: nf4_gemm_sm90.cu).  The output of a launch is a strip of `n_fb x T` token-rows (n_fb = 128-feature blocks
 // of all problems of the launch, T = tokens); CTA c owns the CONTIGUOUS range [start[c], start[c+1]) of that strip and
@@ -133,7 +134,8 @@ constexpr int kFirstDequantWarp = kConsumerWarps;
 constexpr int kNumThreads = 32 * (kFirstDequantWarp + kNumGroups * kGroupWarps);   // 640
 
 // Consumer warpgroup `wg`: all steps of one unit with wgmma N = kN (>= the unit's tokens), then the output stores.
-template <typename T16, int kN, bool kTrans>
+// kOutF16 (bf16 compute only): the output is fp16, the bf16-rounded result rounded again (p.out_f32 is not read).
+template <typename T16, int kN, bool kTrans, bool kOutF16>
 __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, const Sched& sched, int wg, int warp, int lane,
                                              uint32_t smem_base, uint32_t aux, uint32_t& g, float (&acc)[ptx::kWgmmaMaxAcc]) {
   auto in_tile = [&](int s) { return smem_base + uint32_t(s) * kInSlotBytes; };
@@ -202,7 +204,9 @@ __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, con
         const int t = w.t0 + 8 * j + tl + e;
         if (t >= p.T || 8 * j + tl + e >= w.nt) continue;
         const T16 o = round16<T16>(acc[4 * j + 2 * h + e] + bias_v);
-        if (!p.out_f32)
+        if constexpr (kOutF16)
+          static_cast<__half*>(pr.out)[int64_t(t) * pr.ld_out + f] = bf16_to_f16(o);
+        else if (!p.out_f32)
           static_cast<T16*>(pr.out)[int64_t(t) * pr.ld_out + f] = o;
         else   // the 16-bit rounding of the reference's GEMM output first, then widened: one store pass, no cast kernel
           static_cast<float*>(pr.out)[int64_t(t) * pr.ld_out + f] = widen(o);
@@ -210,7 +214,9 @@ __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, con
   }
 }
 
-template <typename T16, bool kTrans, bool kNested>
+// kStateF16: bf16 compute over an fp16 quant state (the double-rounded product table of build_table); kOutF16: see
+// consume_unit.  Both are false for every fp16-compute instantiation.
+template <typename T16, bool kTrans, bool kNested, bool kStateF16, bool kOutF16>
 __global__ void __launch_bounds__(kNumThreads, 1)
 nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p, const __grid_constant__ Sched sched) {
   extern __shared__ uint8_t smem_raw[];
@@ -378,7 +384,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
         float am = fetch.resolve(s_code + pi_cur * 256, offset, valid_cur);
         if (rs_ptr != nullptr) am = __fmul_rn(am, rs_cur);
         Nf4Table tab;
-        build_table<T16>(am, tab);
+        build_table<T16, kStateF16>(am, tab);
         const uint32_t words[8] = {raw0.x, raw0.y, raw0.z, raw0.w, raw1.x, raw1.y, raw1.z, raw1.w};
         ptx::mbar_wait(empty(sa), empty_ph);
         const uint32_t dst = a_tile(sa) + st_base;
@@ -438,14 +444,14 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       const Work w = decode_work(a, cur_end, num_ctas, sched, p, num_kb, has_lora);
       a = w.next;
       switch (w.nt >> 4) {
-        case 1: consume_unit<T16, 16, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 2: consume_unit<T16, 32, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 3: consume_unit<T16, 48, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 4: consume_unit<T16, 64, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 5: consume_unit<T16, 80, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 6: consume_unit<T16, 96, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        case 7: consume_unit<T16, 112, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-        default: consume_unit<T16, 128, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 1: consume_unit<T16, 16, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 2: consume_unit<T16, 32, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 3: consume_unit<T16, 48, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 4: consume_unit<T16, 64, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 5: consume_unit<T16, 80, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 6: consume_unit<T16, 96, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        case 7: consume_unit<T16, 112, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        default: consume_unit<T16, 128, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
       }
     }
   }

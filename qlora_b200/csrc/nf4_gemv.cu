@@ -121,6 +121,16 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
 
 constexpr int kSlabRowBytes = 512;       // x slab of one step: 4 blocks x 64 values x 2 B per token
 
+// Output type of a skinny launch: T16, or fp16 for a bf16-compute launch with fp16 output (kOutF16), which stores the
+// bf16-rounded result rounded to fp16.
+template <typename T16, bool kOutF16>
+using SkinnyOut = typename std::conditional<kOutF16, __half, T16>::type;
+template <typename T16, bool kOutF16>
+__device__ __forceinline__ SkinnyOut<T16, kOutF16> round_out(float v) {
+  if constexpr (kOutF16) return bf16_to_f16(round16<T16>(v));
+  else return round16<T16>(v);
+}
+
 // NT: groups of 8 tokens; kWarps: contraction split inside the CTA; kRing: blocks in flight per thread.
 // (4 warps x 4 blocks in flight measured faster than 8 warps x 2: 11.2 vs 11.5-13.2 us at 4096^2, one token, ncu.)
 //
@@ -138,11 +148,12 @@ constexpr int kSlabRowBytes = 512;       // x slab of one step: 4 blocks x 64 va
 //
 // B operand.  Each thread keeps kRing blocks (32 B of nibbles + absmax statistics each) in flight in registers
 // (the first version waited on one block at a time: ncu long-scoreboard 5.6 stalls / issue).
-template <typename T16, int NT, int kWarps, int kRing, bool kNested>
+// kStateF16: bf16 compute over an fp16 quant state (build_table); kOutF16: see SkinnyOut.
+template <typename T16, int NT, int kWarps, int kRing, bool kNested, bool kStateF16, bool kOutF16>
 __global__ void __launch_bounds__(32 * kWarps, 4)
 nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
                   const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
-                  const float* __restrict__ absmax_f32, const T16* __restrict__ bias, T16* __restrict__ y, int M,
+                  const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y, int M,
                   int N, int K, const T16* __restrict__ lora_u, int ld_u, const T16* __restrict__ lora_v,
                   int lora_r, int64_t ld_x, int64_t ld_y, const float* __restrict__ row_scale) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
@@ -233,7 +244,7 @@ nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed,
       if (row_scale != nullptr) am = __fmul_rn(am, rs);
       if (b >= nblk) am = 0.0f;
       Table tab;
-      build_table<T16>(am, tab);
+      build_table<T16, kStateF16>(am, tab);
       const uint32_t words[8] = {cur.lo.x, cur.lo.y, cur.lo.z, cur.lo.w, cur.hi.x, cur.hi.y, cur.hi.z, cur.hi.w};
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -270,20 +281,22 @@ nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed,
     for (int w = 0; w < kWarps; ++w) v += s_red[(w * NT + nt) * 8 * kRows + i];
     if (lora_r > 0) v += lora_dot(lora_u + int64_t(m) * ld_u, lora_v + int64_t(row) * lora_r, lora_r);
     if (bias != nullptr) v += widen(bias[row]);
-    y[int64_t(m) * ld_y + row] = round16<T16>(v);
+    y[int64_t(m) * ld_y + row] = round_out<T16, kOutF16>(v);
   }
 }
 
 // q's row pitches are resolved (non-zero).  Both instantiations take the full set of state pointers: the nested one reads
 // only absmax_u8 / code256 / absmax2 / offset, the plain one only absmax_f32.
-template <typename T16, int NT, int kWarps, int kRing>
+template <typename T16, bool kStateF16, bool kOutF16, int NT, int kWarps, int kRing>
 static int launch_cfg(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
   constexpr int smem = kWarps * NT * 8 * kSlabRowBytes + 256 * int(sizeof(float));
   static_assert(smem <= 48 * 1024, "static opt-in not needed below 48 KB");
-  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel<T16, NT, kWarps, kRing, true> : nf4_skinny_kernel<T16, NT, kWarps, kRing, false>;
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel<T16, NT, kWarps, kRing, true, kStateF16, kOutF16>
+                                           : nf4_skinny_kernel<T16, NT, kWarps, kRing, false, kStateF16, kOutF16>;
   return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny", static_cast<const T16*>(q.in), q.packed,
-                    q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias), static_cast<T16*>(q.out),
-                    M, N, K, static_cast<const T16*>(q.U), int(q.ld_u), static_cast<const T16*>(q.V), R, q.ld_in, q.ld_out, row_scale);
+                    q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias),
+                    static_cast<SkinnyOut<T16, kOutF16>*>(q.out), M, N, K, static_cast<const T16*>(q.U), int(q.ld_u),
+                    static_cast<const T16*>(q.V), R, q.ld_in, q.ld_out, row_scale);
 }
 
 template <int N>
@@ -302,11 +315,11 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 // look-up costs 2.1 PRMT + 1.3 other ALU instructions per weight at 64 lanes/clk/SM (ncu, 4096x11008: ALU pipe 64 % of its
 // peak while SMs are active, issue slots 44 %, SMs active 71 % of the kernel) — a ceiling of ~2.7 TB/s of packed weights,
 // 0.42 of the HBM roofline, before launch and tail; DESIGN.md 4.3.
-template <typename T16, int kWarps, int kRing, int kBuf, bool kNested>
+template <typename T16, int kWarps, int kRing, int kBuf, bool kNested, bool kStateF16, bool kOutF16>
 __global__ void __launch_bounds__(32 * kWarps, 4)
 nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
                        const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
-                       const float* __restrict__ absmax_f32, const T16* __restrict__ bias, T16* __restrict__ y,
+                       const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y,
                        int N, int K, const T16* __restrict__ lora_u, const T16* __restrict__ lora_v, int lora_r,
                        const float* __restrict__ row_scale) {
   using T2 = typename Vec2<T16>::type;
@@ -392,7 +405,7 @@ nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ pa
       if (row_scale != nullptr) am = __fmul_rn(am, rs);
       if (4 * (warp + kWarps * s) + t >= nblk) am = 0.0f;
       Table tab;
-      build_table<T16>(am, tab);
+      build_table<T16, kStateF16>(am, tab);
       const int buf_off = (u % kBuf) * kSlabRowBytes;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -445,58 +458,66 @@ nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ pa
     for (int w = 0; w < kWarps; ++w) v += s_red[w * kRows + threadIdx.x];
     if (lora_r > 0) v += s_red[kWarps * kRows + threadIdx.x];
     if (bias != nullptr) v += widen(bias[row]);
-    y[row] = round16<T16>(v);
+    y[row] = round_out<T16, kOutF16>(v);
   }
 }
 
 // One token: row pitches do not matter.  State pointers as in launch_cfg.
-template <typename T16, int kWarps, int kRing, int kBuf>
+template <typename T16, bool kStateF16, bool kOutF16, int kWarps, int kRing, int kBuf>
 static int launch_1tok(const qb200_nf4_problem& q, const float* row_scale, int N, int K, int R, cudaStream_t stream) {
   constexpr int kSlabs = kWarps * kBuf * kSlabRowBytes;
   constexpr int kRed = (kWarps + 1) * kRows * int(sizeof(float));
   constexpr int smem = (kSlabs > kRed ? kSlabs : kRed) + 256 * int(sizeof(float));
-  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_1tok<T16, kWarps, kRing, kBuf, true>
-                                           : nf4_skinny_kernel_1tok<T16, kWarps, kRing, kBuf, false>;
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_1tok<T16, kWarps, kRing, kBuf, true, kStateF16, kOutF16>
+                                           : nf4_skinny_kernel_1tok<T16, kWarps, kRing, kBuf, false, kStateF16, kOutF16>;
   return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny_1tok", static_cast<const T16*>(q.in), q.packed,
-                    q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias), static_cast<T16*>(q.out),
-                    N, K, static_cast<const T16*>(q.U), static_cast<const T16*>(q.V), R, row_scale);
+                    q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias),
+                    static_cast<SkinnyOut<T16, kOutF16>*>(q.out), N, K, static_cast<const T16*>(q.U), static_cast<const T16*>(q.V), R,
+                    row_scale);
 }
 
 // 16 tokens per launch (more tokens = more passes over the packed weights, which stay in L2); q's row pitches are resolved.
-template <typename T16>
+template <typename T16, bool kStateF16, bool kOutF16>
 static int launch_chunks(qb200_nf4_problem q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
   constexpr int kChunk = 8 * kMaxNT;
   for (int m0 = 0; m0 < M; m0 += kChunk) {
     const int mc = M - m0 < kChunk ? M - m0 : kChunk;
     int rc;
     if (mc == 1)
-      rc = launch_1tok<T16, 4, 4, 2>(q, row_scale, N, K, R, stream);
+      rc = launch_1tok<T16, kStateF16, kOutF16, 4, 4, 2>(q, row_scale, N, K, R, stream);
     else if (mc <= 8)
-      rc = launch_cfg<T16, 1, 4, 4>(q, row_scale, mc, N, K, R, stream);
+      rc = launch_cfg<T16, kStateF16, kOutF16, 1, 4, 4>(q, row_scale, mc, N, K, R, stream);
     else
-      rc = launch_cfg<T16, 2, 4, 4>(q, row_scale, mc, N, K, R, stream);
+      rc = launch_cfg<T16, kStateF16, kOutF16, 2, 4, 4>(q, row_scale, mc, N, K, R, stream);
     if (rc) return rc;
     q.in = static_cast<const T16*>(q.in) + int64_t(kChunk) * q.ld_in;
     if (q.U) q.U = static_cast<const T16*>(q.U) + int64_t(kChunk) * q.ld_u;
-    q.out = static_cast<T16*>(q.out) + int64_t(kChunk) * q.ld_out;
+    q.out = static_cast<SkinnyOut<T16, kOutF16>*>(q.out) + int64_t(kChunk) * q.ld_out;
   }
   return 0;
 }
 
 }  // namespace skinny
 
-// Internal: forward skinny GEMM, 16 tokens per launch, every 16-bit operand of type `dtype` (bf16 or fp16); optional LoRA term  y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U
+// Internal: forward skinny GEMM, 16 tokens per launch, every 16-bit operand of type `dtype` (bf16 or fp16; a bf16 launch may
+// read an fp16 state's double-rounded weights, state_f16, and write fp16, out_f16); optional LoRA term y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U
 // may be column slices of wider row-major buffers (row pitches ld_in / ld_out / ld_u in elements, 0 = dense); caller has validated
 // pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0, R <= 64, 16-byte aligned in / U rows and V).
-int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, int dtype, cudaStream_t stream) {
+int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, int dtype, int state_f16,
+                      int out_f16, cudaStream_t stream) {
   if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");
   qb200_nf4_problem q = prob;   // advanced by one chunk of tokens per launch
   if (R == 0) q.U = q.V = nullptr;
   if (q.ld_u == 0) q.ld_u = R;
   if (q.ld_in == 0) q.ld_in = K;
   if (q.ld_out == 0) q.ld_out = N;
-  if (dtype == QB200_DTYPE_F16) return skinny::launch_chunks<__half>(q, row_scale, M, N, K, R, stream);
-  return skinny::launch_chunks<__nv_bfloat16>(q, row_scale, M, N, K, R, stream);
+  using BF = __nv_bfloat16;
+  if (dtype == QB200_DTYPE_F16) return skinny::launch_chunks<__half, false, false>(q, row_scale, M, N, K, R, stream);
+  if (state_f16)
+    return out_f16 ? skinny::launch_chunks<BF, true, true>(q, row_scale, M, N, K, R, stream)
+                   : skinny::launch_chunks<BF, true, false>(q, row_scale, M, N, K, R, stream);
+  return out_f16 ? skinny::launch_chunks<BF, false, true>(q, row_scale, M, N, K, R, stream)
+                 : skinny::launch_chunks<BF, false, false>(q, row_scale, M, N, K, R, stream);
 }
 
 }  // namespace qb200

@@ -1,4 +1,5 @@
-// Register-resident product table of one NF4 block: the 16 values  T16_rne(LUT[j] * absmax)  a block can take, kept as
+// Register-resident product table of one NF4 block: the 16 values  T16_rne(LUT[j] * absmax)  a block can take (with an fp16
+// state under bf16 compute: bf16_rne(fp16_rne(LUT[j] * absmax))), kept as
 // low-byte / high-byte planes so that PRMT byte permutes resolve 4 nibbles at a time (2 PRMT per weight, nothing else per
 // weight: no shared-memory look-up, no multiply, no convert).  Shared by the fused GEMM (nf4_gemm_wgmma.cuh), the skinny
 // forward (nf4_gemv.cu) and the standalone dequantize kernel (nf4_quant.cu): all three emit bit-identical weights.
@@ -37,18 +38,30 @@ __device__ __forceinline__ float widen(__nv_bfloat16 v) { return __bfloat162floa
 __device__ __forceinline__ float widen(__half v) { return __half2float(v); }
 __device__ __forceinline__ float2 widen2(__nv_bfloat162 v) { return __bfloat1622float2(v); }
 __device__ __forceinline__ float2 widen2(__half2 v) { return __half22float2(v); }
+// fp16 output of a bf16-compute launch (fp16 activations under bf16 compute): the bf16-rounded result rounded to fp16, which
+// is what `.to(torch.float16)` does to it.
+__device__ __forceinline__ __half bf16_to_f16(__nv_bfloat16 v) { return __float2half_rn(__bfloat162float(v)); }
 
 struct Nf4Table {
   uint32_t tl[4], th[4];  // low / high byte planes of the 16 products
 };
 
-template <typename T16 = __nv_bfloat16>
+// kStateF16 (bf16 compute over an fp16 quant state): every product is first rounded to fp16 (subnormals kept, as
+// cvt.rn.f16x2.f32 does) and widened, then rounded to T16 — the two roundings of `dequantize_4bit(W, fp16 state).to(bf16)`.
+template <typename T16 = __nv_bfloat16, bool kStateF16 = false>
 __device__ __forceinline__ void build_table(float am, Nf4Table& t) {
   constexpr float lut[16] = QB200_NF4_LUT_INIT;
   uint32_t p[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    p[i] = round16x2<T16>(__fmul_rn(lut[2 * i], am), __fmul_rn(lut[2 * i + 1], am));
+    float lo = __fmul_rn(lut[2 * i], am), hi = __fmul_rn(lut[2 * i + 1], am);
+    if constexpr (kStateF16) {
+      const uint32_t h = ptx::cvt_f16x2(lo, hi);
+      const float2 w = __half22float2(*reinterpret_cast<const __half2*>(&h));
+      lo = w.x;
+      hi = w.y;
+    }
+    p[i] = round16x2<T16>(lo, hi);
   }
 #pragma unroll
   for (int g = 0; g < 4; ++g) {

@@ -48,6 +48,8 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaS
 
 // Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16: problem q with its optional LoRA term
 // U[M,R] . V[N,R]^T (R = 0: none) and an optional per-row weight scale row_scale[N] (null: none); every 16-bit operand is of
-// type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16).
-int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, int dtype, cudaStream_t stream);
+// type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16).  bf16 only: state_f16 = 1 reads an fp16 quant state's weights
+// bf16_rn(fp16_rn(LUT[j] * absmax)), out_f16 = 1 writes the bf16-rounded result rounded to fp16.
+int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, int dtype, int state_f16,
+                      int out_f16, cudaStream_t stream);
 }  // namespace qb200

@@ -422,10 +422,11 @@ def dequantize_nf4(A, quant_state=None, absmax=None, out=None, blocksize=64):
 # Fused linear entry points (new exports; SURVEY.md 8b "New export for the fused path")
 # --------------------------------------------------------------------------------------
 
-# Quant-state dtypes whose `dequantize_4bit(...).to(compute_dtype)` is exactly the fused kernels' product table
-# T16_rn(LUT[j] * absmax) for each fused compute dtype.  A bf16 state under fp16 compute rounds twice (bf16, then fp16) and
-# stays on the unfused path; so do fp16 / fp32 states under bf16 compute.
-_FUSED_STATE_DTYPES = {torch.bfloat16: (torch.bfloat16,), torch.float16: (torch.float16, torch.float32)}
+# Quant-state dtypes for which the fused kernels read exactly `dequantize_4bit(...).to(compute_dtype)`, per fused compute
+# dtype: the product table T16_rn(LUT[j] * absmax) for a bf16 or fp32 state under bf16 compute and for an fp16 or fp32 state
+# under fp16 compute, and the double-rounded table bf16_rn(fp16_rn(LUT[j] * absmax)) for an fp16 state under bf16 compute.
+# A bf16 state under fp16 compute stays on the unfused path: no kernel table rounds bf16, then fp16.
+_FUSED_STATE_DTYPES = {torch.bfloat16: (torch.bfloat16, torch.float16, torch.float32), torch.float16: (torch.float16, torch.float32)}
 
 
 def fused_supported(quant_state: QuantState, compute_dtype: torch.dtype) -> bool:
@@ -443,6 +444,12 @@ def fused_supported(quant_state: QuantState, compute_dtype: torch.dtype) -> bool
     return True
 
 
+def double_rounded(quant_state: QuantState, compute_dtype: torch.dtype) -> bool:
+    """Whether the fused kernels round this state's weights twice, bf16_rn(fp16_rn(LUT[j] * absmax)): an fp16 state under
+    bf16 compute.  Problems of one grouped launch agree on it."""
+    return compute_dtype == torch.bfloat16 and quant_state.dtype == torch.float16
+
+
 def as_compute_2d(t: Tensor, dtype: torch.dtype = torch.bfloat16) -> Tensor:
     """`t` as the contiguous [rows, last dim] matrix of the compute dtype (bf16 or fp16) the fused kernels read (cast and
     copied only where needed)."""
@@ -454,8 +461,11 @@ def as_compute_2d(t: Tensor, dtype: torch.dtype = torch.bfloat16) -> Tensor:
 
 def out_dtype_for(in_dtype: torch.dtype, compute_dtype: torch.dtype = torch.bfloat16) -> torch.dtype:
     """What a fused launch writes for activations of `in_dtype`: fp32 for fp32 (the kernel's epilogue widens the result
-    rounded to the compute dtype, as `Linear4bit.forward` returns fp32 for fp32 input), else the compute dtype."""
-    return torch.float32 if in_dtype == torch.float32 else compute_dtype
+    rounded to the compute dtype, as `Linear4bit.forward` returns fp32 for fp32 input), fp16 for fp16 under bf16 compute
+    (the bf16-rounded result rounded to fp16), else the compute dtype."""
+    if in_dtype == torch.float32 or (in_dtype == torch.float16 and compute_dtype == torch.bfloat16):
+        return in_dtype
+    return compute_dtype
 
 
 def _event_begin():
@@ -507,8 +517,10 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group`).
 
     The inputs' dtype (bf16 or fp16) is the compute dtype: U / V / bias are of it too and `out_dtype` is it (the default) or
-    fp32 (the result rounded to it, widened).  fp16 launches go through `qb200_nf4_linear_group_typed`; their event-log kinds
-    end in `_f16`.
+    fp32 (the result rounded to it, widened); under bf16 compute it may also be fp16 (the bf16-rounded result rounded to
+    fp16).  The states share one dtype, which selects the weights: those of `dequantize_4bit(...).to(compute dtype)`.
+    fp16 launches go through `qb200_nf4_linear_group_typed`; their event-log kinds end in `_f16`.  bf16 launches over an fp16
+    state or with an fp16 output go through `qb200_nf4_linear_group_ex`; their kinds end in `_sf16` and / or `_of16`.
 
     forward  (is_bwd=False): out_p = in_p . W_p^T (+bias_p) + U_p . V_p^T for every problem (the inputs may be one tensor);
                              returns the list of outputs.
@@ -530,8 +542,15 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     n_outs = 1 if is_bwd else n
     cdt = inputs[0].dtype
     assert cdt in (torch.bfloat16, torch.float16), f"inputs: bf16 or fp16, got {cdt}"
+    twice = double_rounded(states[0], cdt)
+    assert all(double_rounded(qs, cdt) == twice for qs in states), "grouped problems must share the rounding of their weights"
+    sdt = states[0].dtype
     out_dtype = cdt if out_dtype is None else out_dtype
-    assert out_dtype in (cdt, torch.float32), f"out_dtype: {cdt} or fp32, got {out_dtype}"
+    out_ok = (cdt, torch.float32, torch.float16) if cdt == torch.bfloat16 else (cdt, torch.float32)
+    assert out_dtype in out_ok, f"out_dtype: one of {out_ok}, got {out_dtype}"
+    # bf16 compute over an fp16 state or with an fp16 output: the `_ex` entry point
+    ex = twice or (cdt == torch.bfloat16 and out_dtype == torch.float16)
+    assert not (ex and row_scales is not None), "row scales need a bf16 or fp32 state and a bf16 or fp32 output"
     if outs is None:
         outs = [torch.empty((m, f_out), dtype=out_dtype, device=dev) for _ in range(n_outs)]
     if m == 0:
@@ -594,10 +613,14 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
     what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
-            + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else ""))
+            + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else "")
+            + ("_sf16" if twice else "") + ("_of16" if ex and out_dtype == torch.float16 else ""))
     with torch.cuda.device(dev):
         ev = _event_begin()
-        if cdt == torch.float16:
+        if ex:
+            rc = lib.qb200_nf4_linear_group_ex(int(is_bwd), DTYPE_CODE[cdt], DTYPE_CODE[sdt], n, ct.addressof(probs), r, m, n_out, k_in,
+                                               DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
+        elif cdt == torch.float16:
             rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), _F16_CODE, n, ct.addressof(probs),
                                                   None if scales is None else ct.addressof(scales), r, m, n_out, k_in,
                                                   DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))

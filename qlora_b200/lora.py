@@ -14,8 +14,9 @@ update is ONE extra 16-bit contraction step of the fused kernel, accumulated in 
 
 Only the skinny [M, r] projections stay separate (cuBLAS).  The sum is rounded to the compute dtype once (the unfused
 sequence rounds the base output and the update separately), so results agree with peft's to within one ulp of it.
-The compute dtype is bf16, or fp16 for a base with `compute_dtype=torch.float16` (over an fp16 or fp32 quant state); the
-adapters are of the compute dtype.
+The compute dtype is bf16 (over a bf16 or fp16 quant state), or fp16 for a base with `compute_dtype=torch.float16` (over an
+fp16 or fp32 quant state); the adapters are of the compute dtype.  fp16 activations under bf16 compute, and fp32 states
+under bf16 compute, keep the two-step form, whose base call runs fused through `Linear4bit.forward`.
 
 Dropout (`--lora_dropout 0.1`, scripts/finetune_llama2_guanaco_7b.sh:42): the LoRA branch reads `x_lora = drop(x)`,
 passed as a second input.  Forward is unchanged (U comes from x_lora); in backward the LoRA term of the input gradient
@@ -134,19 +135,24 @@ def _fusable(x, base, lora_a, lora_b) -> bool:
     if base_cdt not in (None, torch.bfloat16, torch.float16):
         return False
     cdt = torch.float16 if base_cdt == torch.float16 else torch.bfloat16
+    # an fp32 state under bf16 compute keeps the two-step form (its base call still runs fused, through Linear4bit): fused,
+    # a grouped dropout step's input gradient rounds differently from per-linear calls by more than their 4e-3 agreement bar
     return (x.is_cuda and x.dtype in (cdt, torch.float32) and base.bias is None and lora_a.dtype == cdt and lora_b.dtype == cdt
-            and qs is not None and F.lora_fused_supported(qs, cdt, lora_a.shape[0]))
+            and qs is not None and not (cdt == torch.bfloat16 and qs.dtype == torch.float32)
+            and F.lora_fused_supported(qs, cdt, lora_a.shape[0]))
 
 
 def _group_fusable(x, bases, lora_as, lora_bs, x_loras) -> bool:
     """Whether 1..3 adapter-wrapped Linear4bit on the input `x` run as ONE fused call: the fused kernel covers each of them,
-    and they share one weight shape, one rank and one quantization form (all nested or all plain), with a dropout input for
-    every linear or for none."""
+    and they share one weight shape, one rank, one quantization form (all nested or all plain) and one rounding of the
+    weights (under bf16 compute: all fp16 states or none), with a dropout input for every linear or for none."""
     if not (1 <= len(bases) <= 3 and all(_fusable(x, b, a, bb) for b, a, bb in zip(bases, lora_as, lora_bs))):
         return False
     states = [b.weight.quant_state for b in bases]
+    cdt = lora_as[0].dtype
     return (len({tuple(qs.shape) for qs in states}) == 1 and len({a.shape[0] for a in lora_as}) == 1
-            and len({qs.nested for qs in states}) == 1 and (x_loras is None or all(t is not None for t in x_loras)))
+            and len({qs.nested for qs in states}) == 1 and len({F.double_rounded(qs, cdt) for qs in states}) == 1
+            and (x_loras is None or all(t is not None for t in x_loras)))
 
 
 class LoraMatMul4Bit(torch.autograd.Function):
@@ -328,8 +334,9 @@ class DoraMatMul4Bit(torch.autograd.Function):
 
 
 def _dora_fusable(x, bases, lora_as, lora_bs, magnitudes, x_loras) -> bool:
-    # bf16 compute only: fp16 DoRA takes the peft form
+    # bf16 compute over bf16 states only: fp16 DoRA, and DoRA over an fp16 or fp32 state, take the peft form
     return (all(a.dtype == torch.bfloat16 for a in lora_as) and _group_fusable(x, bases, lora_as, lora_bs, x_loras)
+            and all(b.weight.quant_state.dtype == torch.bfloat16 for b in bases)
             and all(m.dtype == a.dtype and m.shape == (b.out_features,) for b, a, m in zip(bases, lora_as, magnitudes)))
 
 

@@ -197,11 +197,13 @@ class Linear4bit(nn.Linear):
             raise RuntimeError("Linear4bit weight is not quantized yet: move the module to a CUDA device first (.cuda()/.to('cuda'))")
         qs = self.weight.quant_state
         bias = None if self.bias is None else self.bias.to(self.compute_dtype)
-        if (inp_dtype == torch.float32 and self.compute_dtype in (torch.bfloat16, torch.float16) and x.is_cuda and x.numel() > 0
-                and _autograd.USE_FUSED and F.fused_supported(qs, self.compute_dtype)):
-            # fp32 activations (qlora.py:400-401 keeps the norms in fp32; `qlora.py --fp16` loads the whole model in fp32):
-            # x.to(compute_dtype) and .to(fp32) are folded into the fused node — one input cast, the output cast done by the
-            # kernel epilogue (SURVEY.md 8a row a7)
+        foldable = ((inp_dtype == torch.float32 and self.compute_dtype in (torch.bfloat16, torch.float16))
+                    or (inp_dtype == torch.float16 and self.compute_dtype == torch.bfloat16))
+        if foldable and x.is_cuda and x.numel() > 0 and _autograd.USE_FUSED and F.fused_supported(qs, self.compute_dtype):
+            # fp32 activations (qlora.py:400-401 keeps the norms in fp32; `qlora.py --fp16` loads the whole model in fp32), or
+            # fp16 activations under bf16 compute (an fp16 checkpoint loaded with bnb_4bit_compute_dtype=torch.bfloat16):
+            # x.to(compute_dtype) and .to(inp_dtype) are folded into the fused node — one input cast, the output cast done by
+            # the kernel epilogue (SURVEY.md 8a row a7)
             return matmul_4bit(x, self.weight.t(), bias=bias, quant_state=qs, compute_dtype=self.compute_dtype)
         if self.compute_dtype is not None:
             x = x.to(self.compute_dtype)
