@@ -124,6 +124,13 @@ int qb200_nf4_linear_bwd_dx_lora(const void* dY, const uint8_t* packed, const ui
  * schedule is used.  is_bwd: 0 forward (in = X, out = Y, V = lora_B.weight [N,R]), 1 backward-dX (in = dY, out = dX,
  * V = lora_A.weight [R,K]; bias must be NULL). */
 int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t K, int is_bwd);
+/* Training token counts: at M >= a threshold (default 1536, env QB200_SCRATCH_MIN_M) a call in bf16 compute over a bf16 or fp32
+ * state, with a bf16 or fp32 output and no row scale, writes each of its nprob weights once as bf16 [N,K] into the caller-lent
+ * `workspace` and runs a TMA-fed GEMM over that copy (same weights and summation order as the fused kernel).  This returns
+ * the bytes that needs (nprob*N*K*2), 0 below the threshold; the workspace must be 32-byte aligned.  A call that needs the
+ * scratch and gets a NULL, short or misaligned workspace returns QB200_EINVAL before any launch.  The four entry points above
+ * take no workspace and keep the fused kernel at every M. */
+int64_t qb200_nf4_linear_scratch_size(int nprob, int64_t M, int64_t N, int64_t K, int is_bwd);
 int qb200_nf4_linear_ex(int is_bwd, const void* in, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
                         const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, const void* U,
                         const void* V, int64_t R, void* out, int64_t M, int64_t N, int64_t K, void* workspace,

@@ -36,6 +36,7 @@ _SIGS = {
     "qb200_nf4_linear_fwd_lora": ([_vp] * 10 + [_i64, _vp, _i64, _i64, _i64, _vp], _i32),
     "qb200_nf4_linear_bwd_dx_lora": ([_vp] * 9 + [_i64, _vp, _i64, _i64, _i64, _vp], _i32),
     "qb200_nf4_linear_workspace_size": ([_i64, _i64, _i64, _i32], _i64),
+    "qb200_nf4_linear_scratch_size": ([_i32, _i64, _i64, _i64, _i32], _i64),
     "qb200_adamw32bit_step": ([_vp, _i32, _vp, _vp, _vp, _i64, ct.c_float, ct.c_float, ct.c_float, ct.c_float, ct.c_float, _i32,
                                ct.c_float, _vp], _i32),
     "qb200_adamw32bit_step_dev": ([_vp, _i32, _vp, _vp, _vp, _i64, ct.c_float, ct.c_float, ct.c_float, ct.c_float, ct.c_float, _vp, _vp,

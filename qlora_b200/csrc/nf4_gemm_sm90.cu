@@ -166,13 +166,16 @@ static int plan_ksplit(int T, int F, int C) {
 // step on an H100) and the MMA time (proportional to the tokens: a step is 128 x 64 multiply-adds per token, 4 cycles per
 // token at the dense bf16 rate of an H100 SM), plus the output stores and the pipeline refill between units.  The per-unit
 // terms are estimates, not fitted; QB200_COST_* override every constant for sweeps.
+// The scratch kernel (sc::, 256-token units) has no dequant period: a step costs at least the TMA load of its 16 KB weight
+// tile (QB200_COST_SCRATCH_STEP, about 400 cycles of an SM's share of L2 bandwidth; an estimate), else the MMA time.
 struct CostModel {
   double dq, per_tok, unit, drain_tok;
 };
-static const CostModel& cost_model() {
+static const CostModel& cost_model(int unit_t) {
   static CostModel cm = {double(env_int("QB200_COST_DQ", 1500)), env_int("QB200_COST_TOK_X100", 400) / 100.0,
                          double(env_int("QB200_COST_UNIT", 3000)), env_int("QB200_COST_DRAIN_X100", 1200) / 100.0};
-  return cm;
+  static CostModel cm_scratch = {double(env_int("QB200_COST_SCRATCH_STEP", 400)), cm.per_tok, cm.unit, cm.drain_tok};
+  return unit_t == sc::kUnitT ? cm_scratch : cm;
 }
 static inline double unit_cost(const CostModel& cm, int ntok, int nsteps) {
   const double mma = cm.per_tok * ntok + 24.0;
@@ -180,7 +183,7 @@ static inline double unit_cost(const CostModel& cm, int ntok, int nsteps) {
 }
 
 // Greedy walk over the strip with a per-CTA cycle budget; returns the CTAs used (start[] filled).
-static int walk_ranges(const CostModel& cm, int n_fbg, int t_pad, int nsteps, double budget, int max_ctas, int* start) {
+static int walk_ranges(const CostModel& cm, int unit_t, int n_fbg, int t_pad, int nsteps, double budget, int max_ctas, int* start) {
   const int64_t total = int64_t(n_fbg) * t_pad;
   int64_t pos = 0;
   int c = 0;
@@ -191,7 +194,7 @@ static int walk_ranges(const CostModel& cm, int n_fbg, int t_pad, int nsteps, do
     while (pos < total) {
       const int t0 = int(pos % t_pad);
       int maxlen = t_pad - t0;
-      if (maxlen > kUnitT) maxlen = kUnitT;
+      if (maxlen > unit_t) maxlen = unit_t;
       if (acc + unit_cost(cm, maxlen, nsteps) <= budget) {
         pos += maxlen;
         acc += unit_cost(cm, maxlen, nsteps);
@@ -213,8 +216,9 @@ static int walk_ranges(const CostModel& cm, int n_fbg, int t_pad, int nsteps, do
 }
 
 struct RangeKey {
-  int n_fbg, t_pad, nsteps, ctas;
+  int unit_t, n_fbg, t_pad, nsteps, ctas;
   bool operator<(const RangeKey& o) const {
+    if (unit_t != o.unit_t) return unit_t < o.unit_t;
     if (n_fbg != o.n_fbg) return n_fbg < o.n_fbg;
     if (t_pad != o.t_pad) return t_pad < o.t_pad;
     if (nsteps != o.nsteps) return nsteps < o.nsteps;
@@ -227,29 +231,30 @@ struct RangePlan {
 };
 
 // Balanced contiguous partition of the n_fbg x t_pad strip over the SMs: the smallest per-CTA budget (bisection) for which
-// the greedy walk needs at most `ctas` CTAs.  Plans are cached per shape (host work at capture time only).
-static const RangePlan& plan_ranges(int n_fbg, int t_pad, int nsteps, int ctas) {
+// the greedy walk needs at most `ctas` CTAs, for units of at most `unit_t` tokens (wg::kUnitT or sc::kUnitT).  Plans are
+// cached per shape (host work at capture time only).
+static const RangePlan& plan_ranges(int unit_t, int n_fbg, int t_pad, int nsteps, int ctas) {
   static std::map<RangeKey, RangePlan> cache;
   static std::mutex mu;
   std::lock_guard<std::mutex> lock(mu);
-  const RangeKey key{n_fbg, t_pad, nsteps, ctas};
+  const RangeKey key{unit_t, n_fbg, t_pad, nsteps, ctas};
   auto it = cache.find(key);
   if (it != cache.end()) return it->second;
-  const CostModel& cm = cost_model();
+  const CostModel& cm = cost_model(unit_t);
   RangePlan plan{};
   int tmp[kMaxCtas + 2];
   double lo = 0.0, hi = 0.0;
   for (int f = 0; f < n_fbg; ++f)
-    for (int t = 0; t < t_pad; t += kUnitT) hi += unit_cost(cm, (t_pad - t) < kUnitT ? (t_pad - t) : kUnitT, nsteps);
+    for (int t = 0; t < t_pad; t += unit_t) hi += unit_cost(cm, (t_pad - t) < unit_t ? (t_pad - t) : unit_t, nsteps);
   lo = hi / ctas * 0.5;
   for (int iter = 0; iter < 48; ++iter) {
     const double mid = 0.5 * (lo + hi);
-    if (walk_ranges(cm, n_fbg, t_pad, nsteps, mid, ctas, tmp) <= ctas)
+    if (walk_ranges(cm, unit_t, n_fbg, t_pad, nsteps, mid, ctas, tmp) <= ctas)
       hi = mid;
     else
       lo = mid;
   }
-  plan.n_ctas = walk_ranges(cm, n_fbg, t_pad, nsteps, hi, ctas, plan.start);
+  plan.n_ctas = walk_ranges(cm, unit_t, n_fbg, t_pad, nsteps, hi, ctas, plan.start);
   for (int c = plan.n_ctas + 1; c <= kMaxCtas; ++c) plan.start[c] = plan.start[plan.n_ctas];
   return cache.emplace(key, plan).first->second;
 }
@@ -273,15 +278,15 @@ static auto wgmma_kernel(bool nested) {
   return nested ? nf4_gemm_wgmma_kernel<T16, kTrans, true, kStateF16, kOutF16> : nf4_gemm_wgmma_kernel<T16, kTrans, false, kStateF16, kOutF16>;
 }
 
-template <bool kTrans>
-static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
-  const int T = g.M, F = kTrans ? g.K : g.N, C = kTrans ? g.N : g.K;
-  const bool nested = g.pr[0].absmax_u8 != nullptr;
+// Launch parameters and the activation / LoRA tensor maps of a group, shared by both GEMM kernels; activation and U boxes
+// are `unit_t` rows (the kernel's largest unit).
+template <typename MapsT>
+static int fill_launch(const GroupArgs& g, bool trans, int unit_t, MapsT& maps, Params& p) {
+  const int T = g.M, F = trans ? g.K : g.N, C = trans ? g.N : g.K;
   const CUtensorMapDataType dt = g.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  Maps maps;
-  Params p{};
+  p = Params{};
   p.nprob = g.nprob;
-  p.group_sum = (kTrans && g.nprob > 1) ? 1 : 0;
+  p.group_sum = (trans && g.nprob > 1) ? 1 : 0;
   p.T = T; p.F = F; p.C = C; p.K = g.K; p.N = g.N;
   p.lora_r = g.R;
   p.out_f32 = g.out_f32;
@@ -290,15 +295,15 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     const qb200_nf4_problem& q = g.pr[i];
     const int64_t ld_in = q.ld_in > 0 ? q.ld_in : C;
     int rc = make_map_2d(&maps.in[i], dt, q.in, uint64_t(C), uint64_t(T), uint64_t(ld_in) * 2,
-                         kBlockC, kUnitT, CU_TENSOR_MAP_SWIZZLE_128B);
+                         kBlockC, unit_t, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     if (g.R > 0) {
       // U[T, r] is a K-major B operand like the activation; V is [F, r] (forward, K-major A operand) or [r, F] (dX, MN-major)
       const int64_t ld_u = q.ld_u > 0 ? q.ld_u : g.R;
       rc = make_map_2d(&maps.u[i], dt, q.U, uint64_t(g.R), uint64_t(T), uint64_t(ld_u) * 2, kBlockC,
-                       kUnitT, CU_TENSOR_MAP_SWIZZLE_128B);
+                       unit_t, CU_TENSOR_MAP_SWIZZLE_128B);
       if (rc) return rc;
-      if (!kTrans)
+      if (!trans)
         rc = make_map_2d(&maps.v[i], dt, q.V, uint64_t(g.R), uint64_t(F), uint64_t(g.R) * 2, kBlockC,
                          kBlockF, CU_TENSOR_MAP_SWIZZLE_128B);
       else
@@ -327,6 +332,17 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     maps.v[i] = maps.v[0];
     p.pr[i] = p.pr[0];
   }
+  return 0;
+}
+
+template <bool kTrans>
+static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
+  const int T = g.M, F = kTrans ? g.K : g.N, C = kTrans ? g.N : g.K;
+  const bool nested = g.pr[0].absmax_u8 != nullptr;
+  Maps maps;
+  Params p;
+  const int rc0 = fill_launch(g, kTrans, kUnitT, maps, p);
+  if (rc0) return rc0;
   const int ctas = num_ctas();
   const int n_fb = (F + kUnitF - 1) / kUnitF;
   const int num_kb = (C + kBlockC - 1) / kBlockC;
@@ -350,7 +366,7 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
     const int n_fbg = p.group_sum ? n_fb : n_fb * g.nprob;
     if (int64_t(n_fbg) * sched.t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
     const int nsteps = (p.group_sum ? g.nprob : 1) * (num_kb + (g.R > 0 ? 1 : 0));
-    const RangePlan& plan = plan_ranges(n_fbg, sched.t_pad, nsteps, ctas);
+    const RangePlan& plan = plan_ranges(kUnitT, n_fbg, sched.t_pad, nsteps, ctas);
     n_ctas = plan.n_ctas;
     memcpy(sched.start, plan.start, sizeof(sched.start));
   }
@@ -377,6 +393,62 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   return launch_pdl(g.out_f16 ? splitk_reduce_kernel<BF, true> : splitk_reduce_kernel<BF, false>, blocks, 256, 0, stream, "splitk_reduce",
                     static_cast<const float*>(g.workspace), static_cast<const BF*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32,
                     TF, F, ksplit);
+}
+
+// Smallest token count served by the scratch path (dequantize W once into a bf16 scratch, then the TMA-fed GEMM); smaller
+// counts keep the fused kernel.  QB200_SCRATCH_MIN_M overrides it (tests force either path).
+static int scratch_min_m() {
+  static int v = env_int("QB200_SCRATCH_MIN_M", 1536);
+  return v;
+}
+
+// Bytes of bf16 weight scratch a call of this shape needs: nprob copies of W [N, K], or 0 below the threshold.
+static int64_t scratch_bytes(int64_t nprob, int64_t M, int64_t N, int64_t K) {
+  return M >= scratch_min_m() ? nprob * N * K * 2 : 0;
+}
+
+template <bool kTrans>
+static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
+  const int T = g.M, F = kTrans ? g.K : g.N, C = kTrans ? g.N : g.K;
+  sc::Maps maps;
+  Params p;
+  int rc = fill_launch(g, kTrans, sc::kUnitT, maps, p);
+  if (rc) return rc;
+  const int64_t w_bytes = int64_t(g.N) * g.K * 2;
+  for (int i = 0; i < kMaxProb; ++i) {
+    if (i >= g.nprob) {
+      maps.w[i] = maps.w[0];
+      continue;
+    }
+    // W_p as bf16 [N, K]: box {64, 128} = the K-major forward A tile, {64, 64} = one 64-feature atom of the MN-major dX tile
+    const void* w = static_cast<const uint8_t*>(g.workspace) + i * w_bytes;
+    rc = make_map_2d(&maps.w[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, w, uint64_t(g.K), uint64_t(g.N), uint64_t(g.K) * 2, kBlockC,
+                     kTrans ? kBlockC : kBlockF, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  }
+  Sched sched{};
+  sched.ksplit = 1;
+  sched.t_pad = (T + 15) & ~15;
+  const int n_fb = (F + kUnitF - 1) / kUnitF;
+  const int n_fbg = p.group_sum ? n_fb : n_fb * g.nprob;
+  if (int64_t(n_fbg) * sched.t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
+  const int num_kb = (C + kBlockC - 1) / kBlockC;
+  const int nsteps = (p.group_sum ? g.nprob : 1) * (num_kb + (g.R > 0 ? 1 : 0));
+  const RangePlan& plan = plan_ranges(sc::kUnitT, n_fbg, sched.t_pad, nsteps, num_ctas());
+  memcpy(sched.start, plan.start, sizeof(sched.start));
+  for (int i = 0; i < g.nprob; ++i) {
+    rc = launch_dequant_scratch(g.pr[i], g.N, g.K, static_cast<uint8_t*>(g.workspace) + i * w_bytes, stream);
+    if (rc) return rc;
+  }
+  auto kern = sc::nf4_scratch_gemm_kernel<kTrans>;
+  static bool attr_set[kMaxDevices] = {};
+  if (!attr_set[current_device()]) {
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, sc::kSmemBytes);
+    if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
+    attr_set[current_device()] = true;
+  }
+  return launch_pdl(kern, unsigned(plan.n_ctas), sc::kNumThreads, sc::kSmemBytes, stream,
+                    kTrans ? "nf4_linear_bwd_dx_scratch" : "nf4_linear_fwd_scratch", maps, p, sched);
 }
 
 static int validate_shape(int64_t M, int64_t N, int64_t K) {
@@ -418,9 +490,13 @@ extern "C" int qb200_has_fused_gemm(void) { return 1; }
 // type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16) over a quant state of `state_dtype`, output of `out_dtype` -----------
 // The entry points validate the three dtypes; a bf16 launch reads the double-rounded table only for an fp16 state (a bf16
 // or fp32 state gives the table bf16_rn(LUT[j] * absmax)), and an fp16 launch's table is the same for every state it takes.
+// Training token counts (M >= scratch_min_m()) under bf16 compute over a bf16 or fp32 state, with a bf16 or fp32 output and
+// no row-scale array, take the scratch path: `workspace` must then hold scratch_bytes() of 32-byte aligned device memory.  fp16
+// compute, fp16 states, fp16 outputs and row-scaled launches keep the fused kernel at every token count, as do the four
+// entry points without a workspace (fused_only).
 static int linear_group(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs,
                         const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
-                        int64_t workspace_bytes, void* stream) {
+                        int64_t workspace_bytes, void* stream, bool fused_only = false) {
   if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
   int rc = gemm::validate_shape(M, N, K);
   if (rc) return rc;
@@ -451,6 +527,13 @@ static int linear_group(int is_bwd, int dtype, int state_dtype, int nprob, const
       if (rc) return rc;
     }
     return 0;
+  }
+  if (!fused_only && dtype == QB200_DTYPE_BF16 && !g.state_f16 && !g.out_f16 && !row_scales && M >= gemm::scratch_min_m()) {
+    const int64_t need = gemm::scratch_bytes(nprob, M, N, K);
+    if (workspace == nullptr || workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 32 != 0)
+      return set_error(QB200_EINVAL, "nf4_linear: this token count needs a 32-byte aligned bf16 weight scratch of "
+                                     "qb200_nf4_linear_scratch_size() bytes in `workspace`");
+    return is_bwd ? gemm::launch_scratch_gemm<true>(g, s) : gemm::launch_scratch_gemm<false>(g, s);
   }
   return is_bwd ? gemm::launch_gemm<true>(g, s) : gemm::launch_gemm<false>(g, s);
 }
@@ -506,6 +589,12 @@ extern "C" int qb200_nf4_linear_group_ex(int is_bwd, int dtype, int state_dtype,
   return linear_group(is_bwd, dtype, state_dtype, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
 }
 
+extern "C" int64_t qb200_nf4_linear_scratch_size(int nprob, int64_t M, int64_t N, int64_t K, int is_bwd) {
+  (void)is_bwd;   // the copy is W [N, K] in both directions
+  if (nprob < 1 || nprob > gemm::kMaxProb || M <= 0 || N <= 0 || K <= 0 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX) return 0;
+  return gemm::scratch_bytes(nprob, M, N, K);
+}
+
 extern "C" int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t K, int is_bwd) {
   if (M <= 0 || N <= 0 || K <= 0 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX) return 0;
   const int T = int(M), F = int(is_bwd ? K : N), C = int(is_bwd ? N : K);
@@ -525,19 +614,29 @@ extern "C" int qb200_nf4_linear_ex(int is_bwd, const void* in, const uint8_t* pa
   return qb200_nf4_linear_group(is_bwd, 1, &q, R, M, N, K, QB200_DTYPE_BF16, workspace, workspace_bytes, stream);
 }
 
-// The four specialised entry points are thin wrappers over qb200_nf4_linear_ex (no workspace: un-split schedule).
+// The four specialised entry points take no workspace: un-split schedule, fused kernel at every token count.
+static int linear_no_workspace(int is_bwd, const void* in, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
+                               const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, const void* U,
+                               const void* V, int64_t R, void* out, int64_t M, int64_t N, int64_t K, void* stream) {
+  qb200_nf4_problem q{};
+  q.in = in; q.packed = packed; q.absmax_u8 = absmax_u8; q.code256 = code256; q.absmax2 = absmax2; q.offset = offset;
+  q.absmax_f32 = absmax_f32; q.bias = bias; q.U = U; q.V = V; q.out = out;
+  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, 1, &q, nullptr, R, M, N, K, QB200_DTYPE_BF16, nullptr, 0, stream,
+                      /*fused_only=*/true);
+}
+
 extern "C" int qb200_nf4_linear_fwd(const void* X, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
                                     const float* absmax2, const float* offset, const float* absmax_f32, const void* bias,
                                     void* Y, int64_t M, int64_t N, int64_t K, void* stream) {
-  return qb200_nf4_linear_ex(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, nullptr, nullptr, 0, Y, M, N, K,
-                             nullptr, 0, stream);
+  return linear_no_workspace(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, nullptr, nullptr, 0, Y, M, N, K,
+                             stream);
 }
 
 extern "C" int qb200_nf4_linear_bwd_dx(const void* dY, const uint8_t* packed, const uint8_t* absmax_u8,
                                        const float* code256, const float* absmax2, const float* offset,
                                        const float* absmax_f32, void* dX, int64_t M, int64_t N, int64_t K, void* stream) {
-  return qb200_nf4_linear_ex(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, nullptr, nullptr, 0, dX, M, N, K,
-                             nullptr, 0, stream);
+  return linear_no_workspace(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, nullptr, nullptr, 0, dX, M, N, K,
+                             stream);
 }
 
 // ---- fused LoRA variants (SURVEY.md 8f-1: the caller's low-rank update folded into the same launch) ------------
@@ -546,7 +645,7 @@ extern "C" int qb200_nf4_linear_fwd_lora(const void* X, const uint8_t* packed, c
                                          const void* U, const void* V, int64_t R, void* Y, int64_t M, int64_t N, int64_t K,
                                          void* stream) {
   if (R == 0) return set_error(QB200_EINVAL, "nf4_linear_fwd_lora: R must be > 0");
-  return qb200_nf4_linear_ex(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, U, V, R, Y, M, N, K, nullptr, 0, stream);
+  return linear_no_workspace(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, U, V, R, Y, M, N, K, stream);
 }
 
 extern "C" int qb200_nf4_linear_bwd_dx_lora(const void* dY, const uint8_t* packed, const uint8_t* absmax_u8,
@@ -554,6 +653,5 @@ extern "C" int qb200_nf4_linear_bwd_dx_lora(const void* dY, const uint8_t* packe
                                             const float* absmax_f32, const void* U, const void* Vt, int64_t R, void* dX,
                                             int64_t M, int64_t N, int64_t K, void* stream) {
   if (R == 0) return set_error(QB200_EINVAL, "nf4_linear_bwd_dx_lora: R must be > 0");
-  return qb200_nf4_linear_ex(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, U, Vt, R, dX, M, N, K, nullptr, 0,
-                             stream);
+  return linear_no_workspace(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, U, Vt, R, dX, M, N, K, stream);
 }

@@ -78,7 +78,8 @@ struct Work {
   int split;   // split-K index (0 when the unit covers the whole contraction)
 };
 
-// Decode the unit at cursor `a` of a CTA whose range ends at `end`.
+// Decode the unit at cursor `a` of a CTA whose range ends at `end`; units hold at most kUT tokens.
+template <int kUT = kUnitT>
 __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const Sched& sched, const Params& p, int num_kb,
                                             int has_lora) {
   Work w;
@@ -91,9 +92,9 @@ __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const 
     w.nkb = (num_kb - w.kb0) < per ? (num_kb - w.kb0) : per;
     w.lora = (has_lora && w.split == 0) ? 1 : 0;
     fb = tile / sched.n_tt;
-    w.t0 = (tile - fb * sched.n_tt) * kUnitT;
+    w.t0 = (tile - fb * sched.n_tt) * kUT;
     const int rem = p.T - w.t0;                          // few-token calls issue narrow MMAs and store only what exists
-    w.nt = rem >= kUnitT ? kUnitT : ((rem + 15) & ~15);
+    w.nt = rem >= kUT ? kUT : ((rem + 15) & ~15);
     w.prob = 0;
     w.nseg = 1;
     w.next = a + num_ctas;
@@ -102,7 +103,7 @@ __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const 
     w.t0 = a - fbg * sched.t_pad;
     int ntok = sched.t_pad - w.t0;
     if (end - a < ntok) ntok = end - a;
-    if (ntok > kUnitT) ntok = kUnitT;
+    if (ntok > kUT) ntok = kUT;
     w.next = a + ntok;
     w.nt = ntok;
     if (p.group_sum || p.nprob == 1) {
@@ -132,6 +133,51 @@ constexpr int kGroupWarps = 4;                                  // 128 threads: 
 constexpr int kConsumerWarps = 8;                               // two warpgroups
 constexpr int kFirstDequantWarp = kConsumerWarps;
 constexpr int kNumThreads = 32 * (kFirstDequantWarp + kNumGroups * kGroupWarps);   // 640
+
+// Output of warpgroup `wg`'s 64 x kN part of a unit straight from the accumulator registers (kOutF16: see consume_unit).
+template <typename T16, int kN, bool kOutF16, int kAcc>
+__device__ __forceinline__ void store_unit(const Work& w, const Params& p, const Sched& sched, int wg, int warp, int lane,
+                                           float (&acc)[kAcc]) {
+  // Thread (warp w of the warpgroup, lane l) holds features
+  // f0 + 64 wg + 16 w + l / 4 (+ 8) for tokens t0 + 8 j + 2 (l % 4) + {0, 1}.
+  ptx::grid_dep_wait();   // the output buffer (and bias) may still be in use by an earlier kernel; no-op after the first call
+  if (p.debug & 4) return;
+  const Prob& pr = p.pr[w.prob];
+  const int fa = w.f0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int tl = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int f = fa + 8 * h;
+    if (f >= p.F) continue;
+    if (sched.ksplit > 1) {   // fp32 partial sums into the workspace [ksplit, T, F]; bias is added by the reduce
+      float* ws = p.ws + (int64_t(w.split) * p.T) * p.F + f;
+#pragma unroll
+      for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int t = w.t0 + 8 * j + tl + e;
+          if (t < p.T) ws[int64_t(t) * p.F] = acc[4 * j + 2 * h + e];
+        }
+      continue;
+    }
+    const T16* bias = static_cast<const T16*>(pr.bias);
+    const float bias_v = bias != nullptr ? widen(bias[f]) : 0.0f;
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int t = w.t0 + 8 * j + tl + e;
+        if (t >= p.T || 8 * j + tl + e >= w.nt) continue;
+        const T16 o = round16<T16>(acc[4 * j + 2 * h + e] + bias_v);
+        if constexpr (kOutF16)
+          static_cast<__half*>(pr.out)[int64_t(t) * pr.ld_out + f] = bf16_to_f16(o);
+        else if (!p.out_f32)
+          static_cast<T16*>(pr.out)[int64_t(t) * pr.ld_out + f] = o;
+        else   // the 16-bit rounding of the reference's GEMM output first, then widened: one store pass, no cast kernel
+          static_cast<float*>(pr.out)[int64_t(t) * pr.ld_out + f] = widen(o);
+      }
+  }
+}
 
 // Consumer warpgroup `wg`: all steps of one unit with wgmma N = kN (>= the unit's tokens), then the output stores.
 // kOutF16 (bf16 compute only): the output is fp16, the bf16-rounded result rounded again (p.out_f32 is not read).
@@ -172,46 +218,7 @@ __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, con
   ptx::wgmma_wait<0>(acc);
   __syncwarp();
   if (lane == 0) ptx::mbar_arrive(empty(int((g - 1) % kStages)));
-
-  // Output straight from the accumulator registers.  Thread (warp w of the warpgroup, lane l) holds features
-  // f0 + 64 wg + 16 w + l / 4 (+ 8) for tokens t0 + 8 j + 2 (l % 4) + {0, 1}.
-  ptx::grid_dep_wait();   // the output buffer (and bias) may still be in use by an earlier kernel; no-op after the first call
-  if (p.debug & 4) return;
-  const Prob& pr = p.pr[w.prob];
-  const int fa = w.f0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int tl = 2 * (lane & 3);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int f = fa + 8 * h;
-    if (f >= p.F) continue;
-    if (sched.ksplit > 1) {   // fp32 partial sums into the workspace [ksplit, T, F]; bias is added by the reduce
-      float* ws = p.ws + (int64_t(w.split) * p.T) * p.F + f;
-#pragma unroll
-      for (int j = 0; j < kN / 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int t = w.t0 + 8 * j + tl + e;
-          if (t < p.T) ws[int64_t(t) * p.F] = acc[4 * j + 2 * h + e];
-        }
-      continue;
-    }
-    const T16* bias = static_cast<const T16*>(pr.bias);
-    const float bias_v = bias != nullptr ? widen(bias[f]) : 0.0f;
-#pragma unroll
-    for (int j = 0; j < kN / 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int t = w.t0 + 8 * j + tl + e;
-        if (t >= p.T || 8 * j + tl + e >= w.nt) continue;
-        const T16 o = round16<T16>(acc[4 * j + 2 * h + e] + bias_v);
-        if constexpr (kOutF16)
-          static_cast<__half*>(pr.out)[int64_t(t) * pr.ld_out + f] = bf16_to_f16(o);
-        else if (!p.out_f32)
-          static_cast<T16*>(pr.out)[int64_t(t) * pr.ld_out + f] = o;
-        else   // the 16-bit rounding of the reference's GEMM output first, then widened: one store pass, no cast kernel
-          static_cast<float*>(pr.out)[int64_t(t) * pr.ld_out + f] = widen(o);
-      }
-  }
+  store_unit<T16, kN, kOutF16>(w, p, sched, wg, warp, lane, acc);
 }
 
 // kStateF16: bf16 compute over an fp16 quant state (the double-rounded product table of build_table); kOutF16: see
@@ -457,6 +464,183 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
   }
 }
 
+// =====================================================================================================================
+// TMA-fed GEMM over a bf16 copy of the weights (DESIGN.md 4.1): the scratch path of training token counts.
+//
+// At T >= the scratch threshold the host first writes W_p as bf16 [N, K] into a caller-lent scratch with the bit-exact
+// table kernel (nf4_quant.cu, once per problem and call) and then launches this kernel, so each weight is dequantized once
+// per call instead of once per 128-token unit.  Both operands arrive by TMA and the tensor core sets the pace.
+//
+// Units are 128 features x up to 256 tokens (wgmma m64nNk16, N <= 256, one M=64 half per consumer warpgroup), the same
+// range schedule, work decode, LoRA step, grouped forms and epilogue as the fused kernel above; the A tile of a step is the
+// same 16 KB K-major (forward) or MN-major (dX) tile the dequantizers build, loaded from the scratch instead.  Each output
+// element sums the same products in the same order (NF4 steps in order, then the LoRA step) as the fused kernel.
+//
+// Roles (384 threads): warps 0-7 two consumer warpgroups (setmaxnreg 232: 128 accumulators of m64n256) | warps 8-11 the
+// producer warpgroup (setmaxnreg 40), whose first thread issues every TMA.
+// Barriers: full[s] arrive.expect_tx by the producer + TMA complete_tx of the A and activation tiles -> consumers;
+//           empty[s] 8 consumer-warp arrivals once the step's wgmma group has completed -> producer.
+// Programmatic dependent launch: the producer waits (griddepcontrol.wait) before its first load (the scratch is the output
+// of the dequant kernel launched just before), the consumers before their first output store.
+namespace sc {
+constexpr int kUnitT = 256;                                 // max tokens per unit (wgmma N)
+constexpr int kInSlotBytes = kUnitT * kBlockC * 2;          // 32 KB: one activation block
+constexpr int kStages = 4;                                  // 4 x (16 KB A + 32 KB activations)
+constexpr int kSmemTiles = kStages * (kInSlotBytes + kATileBytes);   // 192 KB
+constexpr int kSmemBytes = kSmemTiles + 1024 + 1024;        // + barriers, + 1 KB alignment of the swizzled tiles
+constexpr int kConsumerWarps = 8;
+constexpr int kNumThreads = 32 * (kConsumerWarps + 4);      // 384
+constexpr int kConsumerRegs = 232;
+constexpr int kProducerRegs = 40;
+static_assert(2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536, "register split exceeds the register file");
+
+struct Maps {
+  CUtensorMap in[kMaxProb];   // activations In_p[T, C], box {64, 256}
+  CUtensorMap u[kMaxProb];    // LoRA U_p[T, r], box {64, 256}
+  CUtensorMap v[kMaxProb];    // LoRA V_p: [F, r] forward, [r, F] dX (as in wg::Maps)
+  CUtensorMap w[kMaxProb];    // bf16 W_p[N, K] in the scratch: box {64, 128} forward (K-major A), {64, 64} dX (MN-major A)
+};
+
+// Consumer warpgroup `wg`: all steps of one unit with wgmma N = kN (>= the unit's tokens), then the output stores.
+template <int kN, bool kTrans>
+__device__ __forceinline__ void consume_unit(const Work& w, const Params& p, const Sched& sched, int wg, int warp, int lane,
+                                             uint32_t smem_base, uint32_t aux, uint32_t& g, float (&acc)[ptx::kWgmmaWideAcc]) {
+  auto in_tile = [&](int s) { return smem_base + uint32_t(s) * kInSlotBytes; };
+  auto a_tile = [&](int s) { return smem_base + uint32_t(kStages) * kInSlotBytes + uint32_t(s) * kATileBytes; };
+  auto full = [&](int s) { return aux + 8u * uint32_t(s); };
+  auto empty = [&](int s) { return aux + 8u * uint32_t(kStages + s); };
+  const int nsteps = w.nseg * (w.nkb + w.lora);
+  for (int kb = 0; kb < nsteps; ++kb, ++g) {
+    const int s = int(g % kStages);
+    ptx::mbar_wait(full(s), (g / kStages) & 1);
+    const uint32_t a_addr = a_tile(s) + uint32_t(wg) * 8192u;
+    const uint64_t a_desc = kTrans ? make_desc_mnmajor_sw128(a_addr, 8192, 1024) : make_desc_kmajor_sw128(a_addr);
+    const uint64_t b_desc = make_desc_kmajor_sw128(in_tile(s));
+    if (!(p.debug & 2)) {
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockC / kMmaK; ++k) {
+        const uint64_t a_adv = kTrans ? uint64_t((k * 2 * 1024) >> 4) : uint64_t((k * kMmaK * 2) >> 4);
+        const uint64_t b_adv = uint64_t((k * kMmaK * 2) >> 4);
+        ptx::wgmma<__nv_bfloat16, kN, kTrans ? 1 : 0>(acc, a_desc + a_adv, b_desc + b_adv, (kb | k) != 0 ? 1u : 0u);
+      }
+      ptx::wgmma_commit();
+    }
+    if (kb > 0) {                 // the previous step's group is complete: release its slot
+      ptx::wgmma_wait<1>(acc);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(empty(int((g - 1) % kStages)));
+    }
+  }
+  ptx::wgmma_wait<0>(acc);
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(empty(int((g - 1) % kStages)));
+  store_unit<__nv_bfloat16, kN, false>(w, p, sched, wg, warp, lane, acc);
+}
+
+template <bool kTrans>
+__global__ void __launch_bounds__(kNumThreads, 1)
+nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p, const __grid_constant__ Sched sched) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+  auto in_tile = [&](int s) { return smem_base + uint32_t(s) * kInSlotBytes; };
+  auto a_tile = [&](int s) { return smem_base + uint32_t(kStages) * kInSlotBytes + uint32_t(s) * kATileBytes; };
+  const uint32_t aux = smem_base + uint32_t(kSmemTiles);
+  auto full = [&](int s) { return aux + 8u * uint32_t(s); };
+  auto empty = [&](int s) { return aux + 8u * uint32_t(kStages + s); };
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_kb = (p.C + kBlockC - 1) / kBlockC;
+  const int has_lora = p.lora_r > 0 ? 1 : 0;
+  const int cur0 = sched.start[blockIdx.x];
+  const int cur_end = sched.start[blockIdx.x + 1];
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < p.nprob; ++i) {
+      ptx::tma_prefetch_desc(&maps.in[i]);
+      ptx::tma_prefetch_desc(&maps.w[i]);
+      if (has_lora) {
+        ptx::tma_prefetch_desc(&maps.u[i]);
+        ptx::tma_prefetch_desc(&maps.v[i]);
+      }
+    }
+    for (int s = 0; s < kStages; ++s) {
+      ptx::mbar_init(full(s), 1);
+      ptx::mbar_init(empty(s), kConsumerWarps);
+    }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+  ptx::grid_dep_launch();
+
+  if (warp >= kConsumerWarps) {
+    // ===================== producer =====================
+    ptx::setmaxnreg_dec<kProducerRegs>();
+    if (warp == kConsumerWarps && ptx::elect_one()) {
+      ptx::grid_dep_wait();   // the scratch, the activations and the adapters are outputs of earlier kernels
+      uint32_t g = 0;
+      for (int a = cur0; a < cur_end;) {
+        const Work w = decode_work<kUnitT>(a, cur_end, gridDim.x, sched, p, num_kb, has_lora);
+        a = w.next;
+        for (int seg = 0; seg < w.nseg; ++seg) {
+          const int pi = p.group_sum ? seg : w.prob;
+          for (int i = 0; i < w.nkb + w.lora; ++i, ++g) {
+            const int s = int(g % kStages);
+            ptx::mbar_wait(empty(s), ((g / kStages) & 1) ^ 1);
+            ptx::mbar_arrive_expect_tx(full(s), kATileBytes + kInSlotBytes);
+            // A: the step's 128 features x 64 contraction of W (or the unit's LoRA V tile), in the consumers' layout
+            const bool lora = i >= w.nkb;
+            const CUtensorMap* am = lora ? &maps.v[pi] : &maps.w[pi];
+            const int c = lora ? 0 : (w.kb0 + i) * kBlockC;
+            if (!kTrans) {
+              ptx::tma_load_2d(a_tile(s), am, full(s), c, w.f0);
+            } else {
+              ptx::tma_load_2d(a_tile(s), am, full(s), w.f0, c);
+              ptx::tma_load_2d(a_tile(s) + 8192u, am, full(s), w.f0 + 64, c);
+            }
+            // activations (LoRA step: U); the box is always 256 rows, rows past T zero-filled, rows past the unit unused
+            ptx::tma_load_2d(in_tile(s), lora ? &maps.u[pi] : &maps.in[pi], full(s), c, w.t0);
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: two warpgroups, wgmma + output =====================
+    ptx::setmaxnreg_inc<kConsumerRegs>();
+    const int wg = warp >> 2;
+    uint32_t g = 0;
+    float acc[ptx::kWgmmaWideAcc];
+#pragma unroll
+    for (int i = 0; i < ptx::kWgmmaWideAcc; ++i) acc[i] = 0.0f;
+    for (int a = cur0; a < cur_end;) {
+      const Work w = decode_work<kUnitT>(a, cur_end, gridDim.x, sched, p, num_kb, has_lora);
+      a = w.next;
+      // N: the unit's tokens rounded up to 16 up to 128, to 32 above
+      if (w.nt <= 128) {
+        switch (w.nt >> 4) {
+          case 1: consume_unit<16, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 2: consume_unit<32, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 3: consume_unit<48, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 4: consume_unit<64, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 5: consume_unit<80, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 6: consume_unit<96, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 7: consume_unit<112, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          default: consume_unit<128, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        }
+      } else {
+        switch ((w.nt + 31) >> 5) {
+          case 5: consume_unit<160, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 6: consume_unit<192, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 7: consume_unit<224, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          default: consume_unit<256, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+        }
+      }
+    }
+  }
+}
+
+}  // namespace sc
 }  // namespace wg
 }  // namespace gemm
 }  // namespace qb200

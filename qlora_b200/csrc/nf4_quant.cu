@@ -460,7 +460,10 @@ __global__ void __launch_bounds__(256) dequantize_nf4_fast_kernel(const uint32_t
 //     is written by exactly one instruction;
 //   * persistent grid (4 CTAs per SM) with the next vector + its absmax statistics prefetched before the current one is
 //     expanded, so loads, look-ups and stores of consecutive iterations overlap.
-template <typename T16, bool NESTED>
+// kPdl: the bf16 weight copy of the scratch GEMM path (launch_dequant_scratch), launched with programmatic stream
+// serialization: it lets the GEMM queued behind it start its prologue at once and issues its first loads (the frozen
+// quant state) before it waits for the previous kernel, whose reads of a recycled scratch buffer must end before any store.
+template <typename T16, bool NESTED, bool kPdl = false>
 __global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __restrict__ packed, const float* __restrict__ absmax,
                                                                  const uint8_t* __restrict__ absmax_u8,
                                                                  const float* __restrict__ code256,
@@ -475,6 +478,7 @@ __global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __
     offset = __ldg(offset_ptr);
     __syncthreads();
   }
+  if constexpr (kPdl) ptx::grid_dep_launch();
   const uint32_t stride = gridDim.x * blockDim.x;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   uint4 w_next;
@@ -492,6 +496,7 @@ __global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __
     }
   };
   fetch(i);
+  if constexpr (kPdl) ptx::grid_dep_wait();
   for (; i < nvec; i += stride) {
     const uint4 w = w_next;
     const float am = NESTED ? nested_absmax(s_code[code_next], scale_next, offset) : scale_next;
@@ -555,6 +560,17 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
 }
 
 static bool valid_blocksize(int bs) { return bs >= 64 && bs <= 4096 && (bs & (bs - 1)) == 0; }
+
+int launch_dequant_scratch(const qb200_nf4_problem& q, int64_t N, int64_t K, void* out, cudaStream_t stream) {
+  const uint32_t nvec = uint32_t(N * K / 32);   // 32 values (16 packed bytes) per vector; blocks of 64, nested blocks of 256
+  int64_t tb = (int64_t(nvec) + 255) / 256;
+  const int64_t tb_max = int64_t(device_sm_count()) * 4;
+  if (tb > tb_max) tb = tb_max;
+  using BF = __nv_bfloat16;
+  const auto kern = q.absmax_u8 != nullptr ? dequantize_nf4_tab_kernel<BF, true, true> : dequantize_nf4_tab_kernel<BF, false, true>;
+  return launch_pdl(kern, unsigned(tb), 256, 0, stream, "dequantize_nf4_scratch", reinterpret_cast<const uint4*>(q.packed),
+                    q.absmax_f32, q.absmax_u8, q.code256, q.absmax2, q.offset, nvec, 1, 8, static_cast<uint8_t*>(out));
+}
 
 }  // namespace qb200
 

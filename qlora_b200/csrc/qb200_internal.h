@@ -52,4 +52,9 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaS
 // bf16_rn(fp16_rn(LUT[j] * absmax)), out_f16 = 1 writes the bf16-rounded result rounded to fp16.
 int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, int dtype, int state_f16,
                       int out_f16, cudaStream_t stream);
+
+// dequantize_4bit(W, state) of problem q as bf16 [N, K] into `out` (32-byte aligned) with the table kernel of nf4_quant.cu —
+// the weights the fused GEMM builds in shared memory, bit for bit (blocks of 64, nested blocks of 256).  Launched with
+// programmatic dependent launch; the scratch GEMM path reads the copy in the next kernel.
+int launch_dequant_scratch(const qb200_nf4_problem& q, int64_t N, int64_t K, void* out, cudaStream_t stream);
 }  // namespace qb200

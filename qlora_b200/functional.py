@@ -611,7 +611,14 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
                 keep.append(sc)
             scales[i] = sc.data_ptr()
     ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
+    # training token counts under bf16 compute (bf16 or fp32 state, bf16 or fp32 output, no row scale): each W is dequantized
+    # once into a bf16 scratch that a TMA-fed GEMM reads; one dequantize launch per problem precedes the GEMM
+    scratch = (lib.qb200_nf4_linear_scratch_size(n, m, n_out, k_in, int(is_bwd))
+               if cdt == torch.bfloat16 and not ex and scales is None else 0)
+    ws_bytes = max(ws_bytes, scratch)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
+    if scratch:
+        LAUNCH_COUNTER[0] += n
     what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
             + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else "")
             + ("_sf16" if twice else "") + ("_of16" if ex and out_dtype == torch.float16 else ""))

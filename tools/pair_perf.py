@@ -6,7 +6,9 @@ bnb-equivalent dequantize + cuBLAS sequence.  One JSON line per case on stdout.
   python tools/pair_perf.py msweep                 # 4096x4096 forward / dX for 17..4096 tokens
   python tools/pair_perf.py one M N K [bwd]        # a single shape (used for env-variable sweeps of the cost model)
 Environment knobs read by the library (static per process): QB200_COST_DQ, QB200_COST_UNIT, QB200_COST_TOK_X100,
-QB200_COST_DRAIN_X100, QB200_SPLITK_MAX_T, QB200_PDL, QB200_DEBUG_FLAGS.
+QB200_COST_DRAIN_X100, QB200_COST_SCRATCH_STEP, QB200_SPLITK_MAX_T, QB200_SCRATCH_MIN_M (17 forces the scratch path of
+training token counts, a huge value the fused kernel: run msweep once each way to place the crossover), QB200_PDL,
+QB200_DEBUG_FLAGS.
 """
 import json
 import os
