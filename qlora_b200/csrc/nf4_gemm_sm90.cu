@@ -12,6 +12,7 @@
 #include <math.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <mutex>
 
@@ -182,15 +183,17 @@ static inline double unit_cost(const CostModel& cm, int ntok, int nsteps) {
   return nsteps * (mma > cm.dq ? mma : cm.dq) + cm.unit + cm.drain_tok * ntok;
 }
 
-// Greedy walk over the strip with a per-CTA cycle budget; returns the CTAs used (start[] filled).
-static int walk_ranges(const CostModel& cm, int unit_t, int n_fbg, int t_pad, int nsteps, double budget, int max_ctas, int* start) {
+// Greedy walk over the strip from token-row pos0 on with a per-CTA cycle budget, CTA c starting from the load base[c] (null:
+// none); returns the CTAs used (start[] filled).
+static int walk_ranges(const CostModel& cm, int unit_t, int n_fbg, int t_pad, int nsteps, int pos0, const double* base,
+                       double budget, int max_ctas, int* start) {
   const int64_t total = int64_t(n_fbg) * t_pad;
-  int64_t pos = 0;
+  int64_t pos = pos0;
   int c = 0;
-  start[0] = 0;
+  start[0] = pos0;
   while (pos < total) {
     if (c == max_ctas) return max_ctas + 1;   // does not fit
-    double acc = 0.0;
+    double acc = base ? base[c] : 0.0;
     while (pos < total) {
       const int t0 = int(pos % t_pad);
       int maxlen = t_pad - t0;
@@ -230,9 +233,35 @@ struct RangePlan {
   int start[kMaxCtas + 1];
 };
 
-// Balanced contiguous partition of the n_fbg x t_pad strip over the SMs: the smallest per-CTA budget (bisection) for which
-// the greedy walk needs at most `ctas` CTAs, for units of at most `unit_t` tokens (wg::kUnitT or sc::kUnitT).  Plans are
-// cached per shape (host work at capture time only).
+// Balanced contiguous partition of the strip's token-rows from pos0 on over the SMs: the smallest per-CTA budget (bisection)
+// for which the greedy walk needs at most `ctas` CTAs, for units of at most `unit_t` tokens (wg::kUnitT or sc::kUnitT), each
+// CTA starting from the load base[c] (null: none).  Returns the CTAs used; start[c] for the unused ones is the strip's end.
+static int balance_ranges(int unit_t, int n_fbg, int t_pad, int nsteps, int ctas, int pos0, const double* base, int* start) {
+  const CostModel& cm = cost_model(unit_t);
+  int tmp[kMaxCtas + 2];
+  const int64_t total = int64_t(n_fbg) * t_pad;
+  double lo = 0.0, hi = 0.0;
+  for (int64_t pos = pos0; pos < total;) {
+    const int t0 = int(pos % t_pad);
+    const int len = (t_pad - t0) < unit_t ? (t_pad - t0) : unit_t;
+    hi += unit_cost(cm, len, nsteps);
+    pos += len;
+  }
+  if (base) hi += *std::max_element(base, base + ctas);
+  lo = hi / ctas * 0.5;
+  for (int iter = 0; iter < 48; ++iter) {
+    const double mid = 0.5 * (lo + hi);
+    if (walk_ranges(cm, unit_t, n_fbg, t_pad, nsteps, pos0, base, mid, ctas, tmp) <= ctas)
+      hi = mid;
+    else
+      lo = mid;
+  }
+  const int n_ctas = walk_ranges(cm, unit_t, n_fbg, t_pad, nsteps, pos0, base, hi, ctas, start);
+  for (int c = n_ctas + 1; c <= kMaxCtas; ++c) start[c] = start[n_ctas];
+  return n_ctas;
+}
+
+// The range schedule of the fused kernel, cached per shape (host work at capture time only).
 static const RangePlan& plan_ranges(int unit_t, int n_fbg, int t_pad, int nsteps, int ctas) {
   static std::map<RangeKey, RangePlan> cache;
   static std::mutex mu;
@@ -240,22 +269,70 @@ static const RangePlan& plan_ranges(int unit_t, int n_fbg, int t_pad, int nsteps
   const RangeKey key{unit_t, n_fbg, t_pad, nsteps, ctas};
   auto it = cache.find(key);
   if (it != cache.end()) return it->second;
-  const CostModel& cm = cost_model(unit_t);
   RangePlan plan{};
-  int tmp[kMaxCtas + 2];
-  double lo = 0.0, hi = 0.0;
-  for (int f = 0; f < n_fbg; ++f)
-    for (int t = 0; t < t_pad; t += unit_t) hi += unit_cost(cm, (t_pad - t) < unit_t ? (t_pad - t) : unit_t, nsteps);
-  lo = hi / ctas * 0.5;
-  for (int iter = 0; iter < 48; ++iter) {
-    const double mid = 0.5 * (lo + hi);
-    if (walk_ranges(cm, unit_t, n_fbg, t_pad, nsteps, mid, ctas, tmp) <= ctas)
-      hi = mid;
-    else
-      lo = mid;
+  plan.n_ctas = balance_ranges(unit_t, n_fbg, t_pad, nsteps, ctas, 0, nullptr, plan.start);
+  return cache.emplace(key, plan).first->second;
+}
+
+// Largest planned cost of a CTA whose load base[c] (null: none) is followed by the range [start[c], start[c+1]).
+static double plan_peak(const CostModel& cm, int unit_t, int t_pad, int nsteps, int ctas, const double* base, const int* start) {
+  double peak = 0.0;
+  for (int c = 0; c < ctas; ++c) {
+    double acc = base ? base[c] : 0.0;
+    for (int pos = start[c]; pos < start[c + 1];) {
+      const int t0 = pos % t_pad;
+      const int len = std::min({t_pad - t0, unit_t, start[c + 1] - pos});
+      acc += unit_cost(cm, len, nsteps);
+      pos += len;
+    }
+    peak = std::max(peak, acc);
   }
-  plan.n_ctas = walk_ranges(cm, unit_t, n_fbg, t_pad, nsteps, hi, ctas, plan.start);
-  for (int c = plan.n_ctas + 1; c <= kMaxCtas; ++c) plan.start[c] = plan.start[plan.n_ctas];
+  return peak;
+}
+
+// The scratch kernel's schedule (sc::Sched, nf4_gemm_wgmma.cuh), cached per shape: full rounds of whole 256-token units,
+// round-robin over the CTAs, then the rest of the strip cut into token ranges with each CTA's round cost as its starting
+// load.  The range schedule of the whole strip (no rounds) is the yardstick and the fall-back: the most rounds are taken
+// for which no CTA's planned cost exceeds that schedule's largest by more than one 16-token step, the resolution of the
+// range schedule itself.  Token counts that are a multiple of 256 keep every full round; ragged ones, whose short last
+// token tiles load the rounds unevenly, may keep fewer.
+struct ScratchPlan {
+  int n_ctas;
+  sc::Sched sched;
+};
+static const ScratchPlan& plan_scratch(int n_fbg, int t_pad, int nsteps, int ctas) {
+  static std::map<RangeKey, ScratchPlan> cache;
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  const RangeKey key{sc::kUnitT, n_fbg, t_pad, nsteps, ctas};
+  auto it = cache.find(key);
+  if (it != cache.end()) return it->second;
+  const CostModel& cm = cost_model(sc::kUnitT);
+  ScratchPlan plan{};
+  sc::Sched& s = plan.sched;
+  s.t_pad = t_pad;
+  s.n_tt = (t_pad + sc::kUnitT - 1) / sc::kUnitT;
+  int range_start[kMaxCtas + 1];
+  const int range_ctas = balance_ranges(sc::kUnitT, n_fbg, t_pad, nsteps, ctas, 0, nullptr, range_start);
+  const double limit = plan_peak(cm, sc::kUnitT, t_pad, nsteps, ctas, nullptr, range_start) + 16 * (cm.per_tok * nsteps + cm.drain_tok);
+  for (int rounds = n_fbg * s.n_tt / ctas; rounds > 0; --rounds) {
+    s.n_rr = rounds * ctas;
+    s.tail0 = (s.n_rr / s.n_tt) * t_pad + (s.n_rr % s.n_tt) * sc::kUnitT;
+    double base[kMaxCtas] = {};
+    for (int u = 0; u < s.n_rr; ++u) {
+      const int t0 = (u % s.n_tt) * sc::kUnitT;
+      base[u % ctas] += unit_cost(cm, std::min(t_pad - t0, sc::kUnitT), nsteps);
+    }
+    balance_ranges(sc::kUnitT, n_fbg, t_pad, nsteps, ctas, s.tail0, base, s.start);
+    if (plan_peak(cm, sc::kUnitT, t_pad, nsteps, ctas, base, s.start) <= limit) {
+      plan.n_ctas = ctas;   // every CTA runs its rounds, whether or not it gets a piece of the tail
+      return cache.emplace(key, plan).first->second;
+    }
+  }
+  s.n_rr = 0;
+  s.tail0 = 0;
+  memcpy(s.start, range_start, sizeof(s.start));
+  plan.n_ctas = range_ctas;
   return cache.emplace(key, plan).first->second;
 }
 
@@ -426,16 +503,13 @@ static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
                      kTrans ? kBlockC : kBlockF, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  Sched sched{};
-  sched.ksplit = 1;
-  sched.t_pad = (T + 15) & ~15;
+  const int t_pad = (T + 15) & ~15;
   const int n_fb = (F + kUnitF - 1) / kUnitF;
   const int n_fbg = p.group_sum ? n_fb : n_fb * g.nprob;
-  if (int64_t(n_fbg) * sched.t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
+  if (int64_t(n_fbg) * t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
   const int num_kb = (C + kBlockC - 1) / kBlockC;
   const int nsteps = (p.group_sum ? g.nprob : 1) * (num_kb + (g.R > 0 ? 1 : 0));
-  const RangePlan& plan = plan_ranges(sc::kUnitT, n_fbg, sched.t_pad, nsteps, num_ctas());
-  memcpy(sched.start, plan.start, sizeof(sched.start));
+  const ScratchPlan& plan = plan_scratch(n_fbg, t_pad, nsteps, num_ctas());
   for (int i = 0; i < g.nprob; ++i) {
     rc = launch_dequant_scratch(g.pr[i], g.N, g.K, static_cast<uint8_t*>(g.workspace) + i * w_bytes, stream);
     if (rc) return rc;
@@ -448,7 +522,7 @@ static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
     attr_set[current_device()] = true;
   }
   return launch_pdl(kern, unsigned(plan.n_ctas), sc::kNumThreads, sc::kSmemBytes, stream,
-                    kTrans ? "nf4_linear_bwd_dx_scratch" : "nf4_linear_fwd_scratch", maps, p, sched);
+                    kTrans ? "nf4_linear_bwd_dx_scratch" : "nf4_linear_fwd_scratch", maps, p, plan.sched);
 }
 
 static int validate_shape(int64_t M, int64_t N, int64_t K) {

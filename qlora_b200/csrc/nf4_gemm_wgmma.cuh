@@ -78,8 +78,7 @@ struct Work {
   int split;   // split-K index (0 when the unit covers the whole contraction)
 };
 
-// Decode the unit at cursor `a` of a CTA whose range ends at `end`; units hold at most kUT tokens.
-template <int kUT = kUnitT>
+// Decode the unit at cursor `a` of a CTA whose range ends at `end`.
 __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const Sched& sched, const Params& p, int num_kb,
                                             int has_lora) {
   Work w;
@@ -92,9 +91,9 @@ __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const 
     w.nkb = (num_kb - w.kb0) < per ? (num_kb - w.kb0) : per;
     w.lora = (has_lora && w.split == 0) ? 1 : 0;
     fb = tile / sched.n_tt;
-    w.t0 = (tile - fb * sched.n_tt) * kUT;
+    w.t0 = (tile - fb * sched.n_tt) * kUnitT;
     const int rem = p.T - w.t0;                          // few-token calls issue narrow MMAs and store only what exists
-    w.nt = rem >= kUT ? kUT : ((rem + 15) & ~15);
+    w.nt = rem >= kUnitT ? kUnitT : ((rem + 15) & ~15);
     w.prob = 0;
     w.nseg = 1;
     w.next = a + num_ctas;
@@ -103,7 +102,7 @@ __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const 
     w.t0 = a - fbg * sched.t_pad;
     int ntok = sched.t_pad - w.t0;
     if (end - a < ntok) ntok = end - a;
-    if (ntok > kUT) ntok = kUT;
+    if (ntok > kUnitT) ntok = kUnitT;
     w.next = a + ntok;
     w.nt = ntok;
     if (p.group_sum || p.nprob == 1) {
@@ -135,8 +134,8 @@ constexpr int kFirstDequantWarp = kConsumerWarps;
 constexpr int kNumThreads = 32 * (kFirstDequantWarp + kNumGroups * kGroupWarps);   // 640
 
 // Output of warpgroup `wg`'s 64 x kN part of a unit straight from the accumulator registers (kOutF16: see consume_unit).
-template <typename T16, int kN, bool kOutF16, int kAcc>
-__device__ __forceinline__ void store_unit(const Work& w, const Params& p, const Sched& sched, int wg, int warp, int lane,
+template <typename T16, int kN, bool kOutF16, int kAcc, typename SchedT>
+__device__ __forceinline__ void store_unit(const Work& w, const Params& p, const SchedT& sched, int wg, int warp, int lane,
                                            float (&acc)[kAcc]) {
   // Thread (warp w of the warpgroup, lane l) holds features
   // f0 + 64 wg + 16 w + l / 4 (+ 8) for tokens t0 + 8 j + 2 (l % 4) + {0, 1}.
@@ -471,10 +470,18 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
 // table kernel (nf4_quant.cu, once per problem and call) and then launches this kernel, so each weight is dequantized once
 // per call instead of once per 128-token unit.  Both operands arrive by TMA and the tensor core sets the pace.
 //
-// Units are 128 features x up to 256 tokens (wgmma m64nNk16, N <= 256, one M=64 half per consumer warpgroup), the same
-// range schedule, work decode, LoRA step, grouped forms and epilogue as the fused kernel above; the A tile of a step is the
-// same 16 KB K-major (forward) or MN-major (dX) tile the dequantizers build, loaded from the scratch instead.  Each output
-// element sums the same products in the same order (NF4 steps in order, then the LoRA step) as the fused kernel.
+// Units are 128 features x up to 256 tokens (wgmma m64nNk16, N <= 256, one M=64 half per consumer warpgroup), with the same
+// LoRA step, grouped forms and epilogue as the fused kernel above; the A tile of a step is the same 16 KB K-major (forward)
+// or MN-major (dX) tile the dequantizers build, loaded from the scratch instead.  Each output element sums the same products
+// in the same order (NF4 steps in order, then the LoRA step) as the fused kernel.
+//
+// Schedule (sc::Sched, host: launch_scratch_gemm).  The units are the 256-token tiles of the n_fb x T strip, numbered
+// feature-block-major with the token tile fastest.  CTA c runs units c, c + P, c + 2P, ... (P = gridDim.x) for the full
+// rounds, so the P units in flight cover about P / n_tt consecutive feature blocks: each 128 x C weight tile is read by
+// n_tt CTAs at about the same time and can stay in L2 between them, instead of coming from HBM once per token tile (a
+// contiguous range per CTA puts the P concurrent units on P different weight tiles, more than L2 holds at C = 4096).  The
+// rest of the strip is cut into token ranges, one per CTA, by the host's range planner, which balances them against each
+// CTA's round cost (plan_scratch).
 //
 // Roles (384 threads): warps 0-7 two consumer warpgroups (setmaxnreg 232: 128 accumulators of m64n256) | warps 8-11 the
 // producer warpgroup (setmaxnreg 40), whose first thread issues every TMA.
@@ -500,6 +507,53 @@ struct Maps {
   CUtensorMap v[kMaxProb];    // LoRA V_p: [F, r] forward, [r, F] dX (as in wg::Maps)
   CUtensorMap w[kMaxProb];    // bf16 W_p[N, K] in the scratch: box {64, 128} forward (K-major A), {64, 64} dX (MN-major A)
 };
+
+// A CTA's cursor is a token-row of the strip: below tail0 it is the first row of one of its round units, from tail0 on it
+// walks the CTA's tail range.  Both rise monotonically, since the tail holds the strip's last units.
+struct Sched {
+  int t_pad;                     // T rounded up to a multiple of 16
+  int n_tt;                      // 256-token tiles per feature block
+  int n_rr;                      // units of the full rounds (a multiple of the CTA count)
+  int tail0;                     // first token-row of unit n_rr, where the tail begins
+  int start[kMaxCtas + 1];       // tail: CTA c owns token-rows [start[c], start[c+1]) of the strip
+  static constexpr int ksplit = 1;   // no split-K (store_unit)
+};
+
+// First token-row of unit u.
+__device__ __forceinline__ int unit_row(int u, const Sched& sched) {
+  return (u / sched.n_tt) * sched.t_pad + (u % sched.n_tt) * kUnitT;
+}
+
+// Decode the unit at cursor `a` of a CTA whose tail range ends at `end`.
+__device__ __forceinline__ Work decode_work(int a, int end, const Sched& sched, const Params& p, int num_kb, int has_lora) {
+  Work w;
+  const int fbg = a / sched.t_pad;
+  w.t0 = a - fbg * sched.t_pad;
+  int ntok = sched.t_pad - w.t0;
+  if (ntok > kUnitT) ntok = kUnitT;
+  if (a < sched.tail0) {         // a round unit: the CTA's next one is gridDim.x units further on, or its tail
+    const int u = fbg * sched.n_tt + w.t0 / kUnitT + int(gridDim.x);
+    w.next = u < sched.n_rr ? unit_row(u, sched) : sched.start[blockIdx.x];
+  } else {
+    if (end - a < ntok) ntok = end - a;
+    w.next = a + ntok;
+  }
+  w.nt = ntok;
+  int fb = fbg;
+  w.prob = 0;
+  w.nseg = p.group_sum ? p.nprob : 1;
+  if (!p.group_sum && p.nprob > 1) {
+    const int n_fb = (p.F + kUnitF - 1) / kUnitF;
+    w.prob = fbg / n_fb;
+    fb = fbg - w.prob * n_fb;
+  }
+  w.f0 = fb * kUnitF;
+  w.split = 0;
+  w.kb0 = 0;
+  w.nkb = num_kb;
+  w.lora = has_lora;
+  return w;
+}
 
 // Consumer warpgroup `wg`: all steps of one unit with wgmma N = kN (>= the unit's tokens), then the output stores.
 template <int kN, bool kTrans>
@@ -553,7 +607,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
   const int lane = threadIdx.x & 31;
   const int num_kb = (p.C + kBlockC - 1) / kBlockC;
   const int has_lora = p.lora_r > 0 ? 1 : 0;
-  const int cur0 = sched.start[blockIdx.x];
+  const int cur0 = sched.n_rr > 0 ? unit_row(int(blockIdx.x), sched) : sched.start[blockIdx.x];
   const int cur_end = sched.start[blockIdx.x + 1];
 
   if (threadIdx.x == 0) {
@@ -581,7 +635,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
       ptx::grid_dep_wait();   // the scratch, the activations and the adapters are outputs of earlier kernels
       uint32_t g = 0;
       for (int a = cur0; a < cur_end;) {
-        const Work w = decode_work<kUnitT>(a, cur_end, gridDim.x, sched, p, num_kb, has_lora);
+        const Work w = decode_work(a, cur_end, sched, p, num_kb, has_lora);
         a = w.next;
         for (int seg = 0; seg < w.nseg; ++seg) {
           const int pi = p.group_sum ? seg : w.prob;
@@ -614,7 +668,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
 #pragma unroll
     for (int i = 0; i < ptx::kWgmmaWideAcc; ++i) acc[i] = 0.0f;
     for (int a = cur0; a < cur_end;) {
-      const Work w = decode_work<kUnitT>(a, cur_end, gridDim.x, sched, p, num_kb, has_lora);
+      const Work w = decode_work(a, cur_end, sched, p, num_kb, has_lora);
       a = w.next;
       // N: the unit's tokens rounded up to 16 up to 128, to 32 above
       if (w.nt <= 128) {
