@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <map>
 #include <mutex>
+#include <set>
 
 namespace qb200 {
 namespace gemm {
@@ -341,18 +342,37 @@ struct GroupArgs {
   const qb200_nf4_problem* pr;
   int R;
   int M, N, K;
-  int out_f32;
-  int f16;                          // 1: every 16-bit operand is fp16, 0: bf16
-  int state_f16;                    // bf16 compute over an fp16 quant state: weights bf16_rn(fp16_rn(LUT[j] * absmax))
-  int out_f16;                      // bf16 compute, fp16 output (the bf16-rounded result rounded to fp16); out_f32 is 0
+  Nf4Variant v;
   void* workspace;
   int64_t workspace_bytes;
   const float* const* row_scales;   // [nprob] or null; an entry may be null (that problem is unscaled)
 };
 
-template <typename T16, bool kTrans, bool kStateF16, bool kOutF16>
-static auto wgmma_kernel(bool nested) {
-  return nested ? nf4_gemm_wgmma_kernel<T16, kTrans, true, kStateF16, kOutF16> : nf4_gemm_wgmma_kernel<T16, kTrans, false, kStateF16, kOutF16>;
+// The dynamic-shared-memory opt-in of `kern`, made once per (device, kernel): the attribute belongs to the device's context.
+static int allow_dynamic_smem(const void* kern, int bytes) {
+  static std::mutex mu;
+  static std::set<std::pair<int, const void*>> done;
+  const std::pair<int, const void*> key{current_device(), kern};
+  std::lock_guard<std::mutex> lock(mu);
+  if (done.count(key)) return 0;
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
+  done.insert(key);
+  return 0;
+}
+
+// The strip that the range and scratch schedules cut into units: n_fbg feature blocks (those of every problem, unless the
+// problems sum into one output) x t_pad token rows, every unit `nsteps` contraction steps long.
+struct Strip {
+  int t_pad, n_fbg, nsteps;
+};
+static int plan_strip(const Params& p, Strip& s) {
+  s.t_pad = (p.T + 15) & ~15;
+  const int n_fb = (p.F + kUnitF - 1) / kUnitF;
+  s.n_fbg = p.group_sum ? n_fb : n_fb * p.nprob;
+  if (int64_t(s.n_fbg) * s.t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
+  s.nsteps = (p.group_sum ? p.nprob : 1) * ((p.C + kBlockC - 1) / kBlockC + (p.lora_r > 0 ? 1 : 0));
+  return 0;
 }
 
 // Launch parameters and the activation / LoRA tensor maps of a group, shared by both GEMM kernels; activation and U boxes
@@ -360,13 +380,13 @@ static auto wgmma_kernel(bool nested) {
 template <typename MapsT>
 static int fill_launch(const GroupArgs& g, bool trans, int unit_t, MapsT& maps, Params& p) {
   const int T = g.M, F = trans ? g.K : g.N, C = trans ? g.N : g.K;
-  const CUtensorMapDataType dt = g.f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMapDataType dt = g.v.kernels == Nf4Kernels::kF16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   p = Params{};
   p.nprob = g.nprob;
   p.group_sum = (trans && g.nprob > 1) ? 1 : 0;
   p.T = T; p.F = F; p.C = C; p.K = g.K; p.N = g.N;
   p.lora_r = g.R;
-  p.out_f32 = g.out_f32;
+  p.out_f32 = g.v.out_f32 ? 1 : 0;
   p.debug = debug_flags();
   for (int i = 0; i < g.nprob; ++i) {
     const qb200_nf4_problem& q = g.pr[i];
@@ -418,11 +438,9 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   const bool nested = g.pr[0].absmax_u8 != nullptr;
   Maps maps;
   Params p;
-  const int rc0 = fill_launch(g, kTrans, kUnitT, maps, p);
-  if (rc0) return rc0;
+  int rc = fill_launch(g, kTrans, kUnitT, maps, p);
+  if (rc) return rc;
   const int ctas = num_ctas();
-  const int n_fb = (F + kUnitF - 1) / kUnitF;
-  const int num_kb = (C + kBlockC - 1) / kBlockC;
   Sched sched{};
   int n_ctas;
   // split-K only for single problems whose caller lent a large enough fp32 workspace [ksplit, T, F]
@@ -433,43 +451,35 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   if (ksplit > 1) {
     sched.ksplit = ksplit;
     sched.n_tt = (T + kUnitT - 1) / kUnitT;
-    sched.n_work = n_fb * sched.n_tt * ksplit;
+    sched.n_work = ((F + kUnitF - 1) / kUnitF) * sched.n_tt * ksplit;
     sched.t_pad = 16;
     n_ctas = sched.n_work < ctas ? sched.n_work : ctas;
     p.ws = static_cast<float*>(g.workspace);
   } else {
+    Strip s;
+    rc = plan_strip(p, s);
+    if (rc) return rc;
     sched.ksplit = 1;
-    sched.t_pad = (T + 15) & ~15;
-    const int n_fbg = p.group_sum ? n_fb : n_fb * g.nprob;
-    if (int64_t(n_fbg) * sched.t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
-    const int nsteps = (p.group_sum ? g.nprob : 1) * (num_kb + (g.R > 0 ? 1 : 0));
-    const RangePlan& plan = plan_ranges(kUnitT, n_fbg, sched.t_pad, nsteps, ctas);
+    sched.t_pad = s.t_pad;
+    const RangePlan& plan = plan_ranges(kUnitT, s.n_fbg, s.t_pad, s.nsteps, ctas);
     n_ctas = plan.n_ctas;
     memcpy(sched.start, plan.start, sizeof(sched.start));
   }
-  using BF = __nv_bfloat16;
-  auto kern = g.f16         ? wgmma_kernel<__half, kTrans, false, false>(nested)
-              : g.state_f16 ? (g.out_f16 ? wgmma_kernel<BF, kTrans, true, true>(nested) : wgmma_kernel<BF, kTrans, true, false>(nested))
-                            : (g.out_f16 ? wgmma_kernel<BF, kTrans, false, true>(nested) : wgmma_kernel<BF, kTrans, false, false>(nested));
-  static bool attr_set[kMaxDevices][2][2][2][2] = {};
-  bool& attr_done = attr_set[current_device()][g.f16][g.state_f16][g.out_f16][nested];
-  if (!attr_done) {   // the dynamic-smem opt-in is per device and instantiation
-    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-    attr_done = true;
-  }
-  const int rc = launch_pdl(kern, unsigned(n_ctas), kNumThreads, kSmemBytes, stream, kTrans ? "nf4_linear_bwd_dx" : "nf4_linear_fwd",
-                            maps, p, sched);
-  if (rc || ksplit == 1) return rc;
-  const int64_t TF = int64_t(T) * F;
-  const int64_t nthreads = TF / 4;
-  const unsigned blocks = unsigned((nthreads + 255) / 256);
-  if (g.f16)
-    return launch_pdl(splitk_reduce_kernel<__half, false>, blocks, 256, 0, stream, "splitk_reduce", static_cast<const float*>(g.workspace),
-                      static_cast<const __half*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32, TF, F, ksplit);
-  return launch_pdl(g.out_f16 ? splitk_reduce_kernel<BF, true> : splitk_reduce_kernel<BF, false>, blocks, 256, 0, stream, "splitk_reduce",
-                    static_cast<const float*>(g.workspace), static_cast<const BF*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out, p.out_f32,
-                    TF, F, ksplit);
+  return with_nf4_types(g.v.kernels, [&](auto t) {
+    using Ty = decltype(t);
+    using T16 = typename Ty::T16;
+    const auto kern = nested ? nf4_gemm_wgmma_kernel<T16, kTrans, true, Ty::kStateF16, Ty::kOutF16>
+                             : nf4_gemm_wgmma_kernel<T16, kTrans, false, Ty::kStateF16, Ty::kOutF16>;
+    rc = allow_dynamic_smem(reinterpret_cast<const void*>(kern), kSmemBytes);
+    if (rc) return rc;
+    rc = launch_pdl(kern, unsigned(n_ctas), kNumThreads, kSmemBytes, stream, kTrans ? "nf4_linear_bwd_dx" : "nf4_linear_fwd", maps,
+                    p, sched);
+    if (rc || ksplit == 1) return rc;
+    const int64_t TF = int64_t(T) * F;
+    return launch_pdl(splitk_reduce_kernel<T16, Ty::kOutF16>, unsigned((TF / 4 + 255) / 256), 256, 0, stream, "splitk_reduce",
+                      static_cast<const float*>(g.workspace), static_cast<const T16*>(p.pr[0].bias), p.pr[0].out, p.pr[0].ld_out,
+                      p.out_f32, TF, F, ksplit);
+  });
 }
 
 // Smallest token count served by the scratch path (dequantize W once into a bf16 scratch, then the TMA-fed GEMM); smaller
@@ -486,7 +496,6 @@ static int64_t scratch_bytes(int64_t nprob, int64_t M, int64_t N, int64_t K) {
 
 template <bool kTrans>
 static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
-  const int T = g.M, F = kTrans ? g.K : g.N, C = kTrans ? g.N : g.K;
   sc::Maps maps;
   Params p;
   int rc = fill_launch(g, kTrans, sc::kUnitT, maps, p);
@@ -503,24 +512,17 @@ static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
                      kTrans ? kBlockC : kBlockF, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  const int t_pad = (T + 15) & ~15;
-  const int n_fb = (F + kUnitF - 1) / kUnitF;
-  const int n_fbg = p.group_sum ? n_fb : n_fb * g.nprob;
-  if (int64_t(n_fbg) * t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
-  const int num_kb = (C + kBlockC - 1) / kBlockC;
-  const int nsteps = (p.group_sum ? g.nprob : 1) * (num_kb + (g.R > 0 ? 1 : 0));
-  const ScratchPlan& plan = plan_scratch(n_fbg, t_pad, nsteps, num_ctas());
+  Strip s;
+  rc = plan_strip(p, s);
+  if (rc) return rc;
+  const ScratchPlan& plan = plan_scratch(s.n_fbg, s.t_pad, s.nsteps, num_ctas());
   for (int i = 0; i < g.nprob; ++i) {
     rc = launch_dequant_scratch(g.pr[i], g.N, g.K, static_cast<uint8_t*>(g.workspace) + i * w_bytes, stream);
     if (rc) return rc;
   }
-  auto kern = sc::nf4_scratch_gemm_kernel<kTrans>;
-  static bool attr_set[kMaxDevices] = {};
-  if (!attr_set[current_device()]) {
-    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, sc::kSmemBytes);
-    if (e != cudaSuccess) return set_error(int(e), "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
-    attr_set[current_device()] = true;
-  }
+  const auto kern = sc::nf4_scratch_gemm_kernel<kTrans>;
+  rc = allow_dynamic_smem(reinterpret_cast<const void*>(kern), sc::kSmemBytes);
+  if (rc) return rc;
   return launch_pdl(kern, unsigned(plan.n_ctas), sc::kNumThreads, sc::kSmemBytes, stream,
                     kTrans ? "nf4_linear_bwd_dx_scratch" : "nf4_linear_fwd_scratch", maps, p, plan.sched);
 }
@@ -560,17 +562,37 @@ using namespace qb200;
 
 extern "C" int qb200_has_fused_gemm(void) { return 1; }
 
+// The kernels for compute `dtype` over a quant state of `state_dtype` writing `out_dtype`: the one list of supported
+// combinations.  bf16 compute takes a bf16, fp16 or fp32 state and writes bf16, fp32 or fp16; it reads the double-rounded table
+// only for an fp16 state (a bf16 or fp32 state gives the table bf16_rn(LUT[j] * absmax)).  fp16 compute takes an fp16 or fp32
+// state, whose table is the same, and writes fp16 or fp32.  False for every other combination.
+static bool nf4_variant(int dtype, int state_dtype, int out_dtype, Nf4Variant& v) {
+  const bool state_f16 = state_dtype == QB200_DTYPE_F16, out_f16 = out_dtype == QB200_DTYPE_F16;
+  v.out_f32 = out_dtype == QB200_DTYPE_F32;
+  if (dtype == QB200_DTYPE_F16) {
+    v.kernels = Nf4Kernels::kF16;
+    return (state_f16 || state_dtype == QB200_DTYPE_F32) && (out_f16 || v.out_f32);
+  }
+  v.kernels = state_f16 ? (out_f16 ? Nf4Kernels::kBf16StateF16OutF16 : Nf4Kernels::kBf16StateF16)
+                        : (out_f16 ? Nf4Kernels::kBf16OutF16 : Nf4Kernels::kBf16);
+  return dtype == QB200_DTYPE_BF16 && (state_f16 || state_dtype == QB200_DTYPE_F32 || state_dtype == QB200_DTYPE_BF16) &&
+         (out_f16 || v.out_f32 || out_dtype == QB200_DTYPE_BF16);
+}
+
 // ---- general entry point: 1..3 problems of one shape in ONE launch, each with an optional row scale; 16-bit operands of
 // type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16) over a quant state of `state_dtype`, output of `out_dtype` -----------
-// The entry points validate the three dtypes; a bf16 launch reads the double-rounded table only for an fp16 state (a bf16
-// or fp32 state gives the table bf16_rn(LUT[j] * absmax)), and an fp16 launch's table is the same for every state it takes.
 // Training token counts (M >= scratch_min_m()) under bf16 compute over a bf16 or fp32 state, with a bf16 or fp32 output and
 // no row-scale array, take the scratch path: `workspace` must then hold scratch_bytes() of 32-byte aligned device memory.  fp16
 // compute, fp16 states, fp16 outputs and row-scaled launches keep the fused kernel at every token count, as do the four
 // entry points without a workspace (fused_only).
-static int linear_group(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs,
-                        const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
+static int linear_group(int is_bwd, int dtype, int state_dtype, int out_dtype, int nprob, const qb200_nf4_problem* probs,
+                        const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, void* workspace,
                         int64_t workspace_bytes, void* stream, bool fused_only = false) {
+  Nf4Variant v;
+  if (!nf4_variant(dtype, state_dtype, out_dtype, v))
+    return set_error(QB200_EINVAL, "nf4_linear_group_ex: unsupported (dtype, state_dtype, out_dtype): bf16 compute takes a bf16, fp16 "
+                                   "or fp32 state and writes bf16, fp32 or fp16; fp16 compute takes an fp16 or fp32 state and "
+                                   "writes fp16 or fp32");
   if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
   int rc = gemm::validate_shape(M, N, K);
   if (rc) return rc;
@@ -585,24 +607,20 @@ static int linear_group(int is_bwd, int dtype, int state_dtype, int nprob, const
     if (row_scales && reinterpret_cast<uintptr_t>(row_scales[i]) % 4 != 0)
       return set_error(QB200_EINVAL, "nf4_linear_group_scaled: row scales must be 4-byte aligned fp32");
   }
-  const bool bf16 = dtype == QB200_DTYPE_BF16;
-  gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), out_dtype == QB200_DTYPE_F32 ? 1 : 0,
-                    dtype == QB200_DTYPE_F16 ? 1 : 0, bf16 && state_dtype == QB200_DTYPE_F16 ? 1 : 0,
-                    bf16 && out_dtype == QB200_DTYPE_F16 ? 1 : 0, workspace, workspace_bytes, row_scales};
+  const gemm::GroupArgs g{nprob, probs, int(R), int(M), int(N), int(K), v, workspace, workspace_bytes, row_scales};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // forward with at most 16 tokens and a 16-bit output: warp-level skinny kernels (nf4_gemv.cu), SURVEY.md 8f-2 — with LoRA
   // operands too (the reference generates with the adapters attached: base GEMV + peft's two small matmuls; here the U . V^T
   // term is the kernel's epilogue)
   // A grouped forward (q/k/v, gate/up) is nprob launches of them, chained by programmatic dependent launch.
-  if (!is_bwd && out_dtype != QB200_DTYPE_F32 && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
+  if (!is_bwd && !v.out_f32 && M <= gemm::skinny_max_m() && !(gemm::debug_flags() & 8)) {
     for (int i = 0; i < nprob; ++i) {
-      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), dtype, g.state_f16,
-                             g.out_f16, s);
+      rc = launch_nf4_skinny(probs[i], row_scales ? row_scales[i] : nullptr, int(M), int(N), int(K), int(R), v.kernels, s);
       if (rc) return rc;
     }
     return 0;
   }
-  if (!fused_only && dtype == QB200_DTYPE_BF16 && !g.state_f16 && !g.out_f16 && !row_scales && M >= gemm::scratch_min_m()) {
+  if (!fused_only && v.kernels == Nf4Kernels::kBf16 && !row_scales && M >= gemm::scratch_min_m()) {
     const int64_t need = gemm::scratch_bytes(nprob, M, N, K);
     if (workspace == nullptr || workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 32 != 0)
       return set_error(QB200_EINVAL, "nf4_linear: this token count needs a 32-byte aligned bf16 weight scratch of "
@@ -612,55 +630,36 @@ static int linear_group(int is_bwd, int dtype, int state_dtype, int nprob, const
   return is_bwd ? gemm::launch_gemm<true>(g, s) : gemm::launch_gemm<false>(g, s);
 }
 
-// dtype / out_dtype rule of the bf16 and typed entry points: the operand dtype is bf16 or fp16, the output is of it or fp32
-static int check_typed_dtypes(int dtype, int out_dtype) {
-  if (dtype != QB200_DTYPE_BF16 && dtype != QB200_DTYPE_F16)
+extern "C" int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs,
+                                            const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
+  Nf4Variant v;
+  if (!nf4_variant(dtype, dtype, dtype, v))
     return set_error(QB200_EINVAL, "nf4_linear_group_typed: dtype must be 2 (bf16) or 1 (fp16)");
   if (out_dtype != dtype && out_dtype != QB200_DTYPE_F32)
     return set_error(QB200_EINVAL, dtype == QB200_DTYPE_BF16 ? "nf4_linear_group: out_dtype must be 2 (bf16) or 0 (fp32)"
                                                              : "nf4_linear_group_typed: out_dtype must be 1 (fp16) or 0 (fp32)");
-  return 0;
+  return linear_group(is_bwd, dtype, dtype, out_dtype, nprob, probs, row_scales, R, M, N, K, workspace, workspace_bytes, stream);
 }
 
 extern "C" int qb200_nf4_linear_group(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M, int64_t N,
                                       int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream) {
-  const int rc = check_typed_dtypes(QB200_DTYPE_BF16, out_dtype);
-  if (rc) return rc;
-  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace,
-                      workspace_bytes, stream);
+  return qb200_nf4_linear_group_typed(is_bwd, QB200_DTYPE_BF16, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace,
+                                      workspace_bytes, stream);
 }
 
 extern "C" int qb200_nf4_linear_group_scaled(int is_bwd, int nprob, const qb200_nf4_problem* probs, const float* const* row_scales,
                                              int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
                                              int64_t workspace_bytes, void* stream) {
   if (!row_scales) return set_error(QB200_EINVAL, "nf4_linear_group_scaled: null row-scale array (NULL entries mean unscaled)");
-  const int rc = check_typed_dtypes(QB200_DTYPE_BF16, out_dtype);
-  if (rc) return rc;
-  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace,
-                      workspace_bytes, stream);
-}
-
-extern "C" int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_nf4_problem* probs,
-                                            const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype,
-                                            void* workspace, int64_t workspace_bytes, void* stream) {
-  const int rc = check_typed_dtypes(dtype, out_dtype);
-  if (rc) return rc;
-  return linear_group(is_bwd, dtype, dtype, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  return qb200_nf4_linear_group_typed(is_bwd, QB200_DTYPE_BF16, nprob, probs, row_scales, R, M, N, K, out_dtype, workspace,
+                                      workspace_bytes, stream);
 }
 
 extern "C" int qb200_nf4_linear_group_ex(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int64_t R,
                                          int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
                                          void* stream) {
-  const bool f32_or_f16_state = state_dtype == QB200_DTYPE_F32 || state_dtype == QB200_DTYPE_F16;
-  const bool ok = dtype == QB200_DTYPE_BF16
-                      ? (f32_or_f16_state || state_dtype == QB200_DTYPE_BF16) &&
-                            (out_dtype == QB200_DTYPE_BF16 || out_dtype == QB200_DTYPE_F32 || out_dtype == QB200_DTYPE_F16)
-                      : dtype == QB200_DTYPE_F16 && f32_or_f16_state && (out_dtype == QB200_DTYPE_F16 || out_dtype == QB200_DTYPE_F32);
-  if (!ok)
-    return set_error(QB200_EINVAL, "nf4_linear_group_ex: unsupported (dtype, state_dtype, out_dtype): bf16 compute takes a bf16, fp16 "
-                                   "or fp32 state and writes bf16, fp32 or fp16; fp16 compute takes an fp16 or fp32 state and "
-                                   "writes fp16 or fp32");
-  return linear_group(is_bwd, dtype, state_dtype, nprob, probs, nullptr, R, M, N, K, out_dtype, workspace, workspace_bytes, stream);
+  return linear_group(is_bwd, dtype, state_dtype, out_dtype, nprob, probs, nullptr, R, M, N, K, workspace, workspace_bytes, stream);
 }
 
 extern "C" int64_t qb200_nf4_linear_scratch_size(int nprob, int64_t M, int64_t N, int64_t K, int is_bwd) {
@@ -678,39 +677,39 @@ extern "C" int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t
   return ks > 1 ? int64_t(ks) * T * F * 4 : 0;
 }
 
+// One bf16 problem: the single-problem entry points.  The four that take no workspace pass fused_only: un-split schedule,
+// fused kernel at every token count.
+static int linear_one(int is_bwd, const void* in, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
+                      const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, const void* U,
+                      const void* V, int64_t R, void* out, int64_t M, int64_t N, int64_t K, void* workspace, int64_t workspace_bytes,
+                      void* stream, bool fused_only) {
+  qb200_nf4_problem q{};
+  q.in = in; q.packed = packed; q.absmax_u8 = absmax_u8; q.code256 = code256; q.absmax2 = absmax2; q.offset = offset;
+  q.absmax_f32 = absmax_f32; q.bias = bias; q.U = U; q.V = V; q.out = out;
+  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, QB200_DTYPE_BF16, 1, &q, nullptr, R, M, N, K, workspace,
+                      workspace_bytes, stream, fused_only);
+}
+
 extern "C" int qb200_nf4_linear_ex(int is_bwd, const void* in, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
                                    const float* absmax2, const float* offset, const float* absmax_f32, const void* bias,
                                    const void* U, const void* V, int64_t R, void* out, int64_t M, int64_t N, int64_t K,
                                    void* workspace, int64_t workspace_bytes, void* stream) {
-  qb200_nf4_problem q{};
-  q.in = in; q.packed = packed; q.absmax_u8 = absmax_u8; q.code256 = code256; q.absmax2 = absmax2; q.offset = offset;
-  q.absmax_f32 = absmax_f32; q.bias = bias; q.U = U; q.V = V; q.out = out;
-  return qb200_nf4_linear_group(is_bwd, 1, &q, R, M, N, K, QB200_DTYPE_BF16, workspace, workspace_bytes, stream);
-}
-
-// The four specialised entry points take no workspace: un-split schedule, fused kernel at every token count.
-static int linear_no_workspace(int is_bwd, const void* in, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
-                               const float* absmax2, const float* offset, const float* absmax_f32, const void* bias, const void* U,
-                               const void* V, int64_t R, void* out, int64_t M, int64_t N, int64_t K, void* stream) {
-  qb200_nf4_problem q{};
-  q.in = in; q.packed = packed; q.absmax_u8 = absmax_u8; q.code256 = code256; q.absmax2 = absmax2; q.offset = offset;
-  q.absmax_f32 = absmax_f32; q.bias = bias; q.U = U; q.V = V; q.out = out;
-  return linear_group(is_bwd, QB200_DTYPE_BF16, QB200_DTYPE_BF16, 1, &q, nullptr, R, M, N, K, QB200_DTYPE_BF16, nullptr, 0, stream,
-                      /*fused_only=*/true);
+  return linear_one(is_bwd, in, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, U, V, R, out, M, N, K, workspace,
+                    workspace_bytes, stream, false);
 }
 
 extern "C" int qb200_nf4_linear_fwd(const void* X, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
                                     const float* absmax2, const float* offset, const float* absmax_f32, const void* bias,
                                     void* Y, int64_t M, int64_t N, int64_t K, void* stream) {
-  return linear_no_workspace(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, nullptr, nullptr, 0, Y, M, N, K,
-                             stream);
+  return linear_one(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, nullptr, nullptr, 0, Y, M, N, K, nullptr, 0,
+                    stream, true);
 }
 
 extern "C" int qb200_nf4_linear_bwd_dx(const void* dY, const uint8_t* packed, const uint8_t* absmax_u8,
                                        const float* code256, const float* absmax2, const float* offset,
                                        const float* absmax_f32, void* dX, int64_t M, int64_t N, int64_t K, void* stream) {
-  return linear_no_workspace(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, nullptr, nullptr, 0, dX, M, N, K,
-                             stream);
+  return linear_one(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, nullptr, nullptr, 0, dX, M, N, K, nullptr,
+                    0, stream, true);
 }
 
 // ---- fused LoRA variants (SURVEY.md 8f-1: the caller's low-rank update folded into the same launch) ------------
@@ -719,7 +718,7 @@ extern "C" int qb200_nf4_linear_fwd_lora(const void* X, const uint8_t* packed, c
                                          const void* U, const void* V, int64_t R, void* Y, int64_t M, int64_t N, int64_t K,
                                          void* stream) {
   if (R == 0) return set_error(QB200_EINVAL, "nf4_linear_fwd_lora: R must be > 0");
-  return linear_no_workspace(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, U, V, R, Y, M, N, K, stream);
+  return linear_one(0, X, packed, absmax_u8, code256, absmax2, offset, absmax_f32, bias, U, V, R, Y, M, N, K, nullptr, 0, stream, true);
 }
 
 extern "C" int qb200_nf4_linear_bwd_dx_lora(const void* dY, const uint8_t* packed, const uint8_t* absmax_u8,
@@ -727,5 +726,6 @@ extern "C" int qb200_nf4_linear_bwd_dx_lora(const void* dY, const uint8_t* packe
                                             const float* absmax_f32, const void* U, const void* Vt, int64_t R, void* dX,
                                             int64_t M, int64_t N, int64_t K, void* stream) {
   if (R == 0) return set_error(QB200_EINVAL, "nf4_linear_bwd_dx_lora: R must be > 0");
-  return linear_no_workspace(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, U, Vt, R, dX, M, N, K, stream);
+  return linear_one(1, dY, packed, absmax_u8, code256, absmax2, offset, absmax_f32, nullptr, U, Vt, R, dX, M, N, K, nullptr, 0, stream,
+                    true);
 }

@@ -499,25 +499,22 @@ static int launch_chunks(qb200_nf4_problem q, const float* row_scale, int M, int
 
 }  // namespace skinny
 
-// Internal: forward skinny GEMM, 16 tokens per launch, every 16-bit operand of type `dtype` (bf16 or fp16; a bf16 launch may
-// read an fp16 state's double-rounded weights, state_f16, and write fp16, out_f16); optional LoRA term y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U
-// may be column slices of wider row-major buffers (row pitches ld_in / ld_out / ld_u in elements, 0 = dense); caller has validated
+// Internal: forward skinny GEMM, 16 tokens per launch, with the skinny kernels of `kernels`; optional LoRA term
+// y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U may be column
+// slices of wider row-major buffers (row pitches ld_in / ld_out / ld_u in elements, 0 = dense); caller has validated
 // pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0, R <= 64, 16-byte aligned in / U rows and V).
-int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, int dtype, int state_f16,
-                      int out_f16, cudaStream_t stream) {
+int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, Nf4Kernels kernels,
+                      cudaStream_t stream) {
   if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");
   qb200_nf4_problem q = prob;   // advanced by one chunk of tokens per launch
   if (R == 0) q.U = q.V = nullptr;
   if (q.ld_u == 0) q.ld_u = R;
   if (q.ld_in == 0) q.ld_in = K;
   if (q.ld_out == 0) q.ld_out = N;
-  using BF = __nv_bfloat16;
-  if (dtype == QB200_DTYPE_F16) return skinny::launch_chunks<__half, false, false>(q, row_scale, M, N, K, R, stream);
-  if (state_f16)
-    return out_f16 ? skinny::launch_chunks<BF, true, true>(q, row_scale, M, N, K, R, stream)
-                   : skinny::launch_chunks<BF, true, false>(q, row_scale, M, N, K, R, stream);
-  return out_f16 ? skinny::launch_chunks<BF, false, true>(q, row_scale, M, N, K, R, stream)
-                 : skinny::launch_chunks<BF, false, false>(q, row_scale, M, N, K, R, stream);
+  return with_nf4_types(kernels, [&](auto t) {
+    using Ty = decltype(t);
+    return skinny::launch_chunks<typename Ty::T16, Ty::kStateF16, Ty::kOutF16>(q, row_scale, M, N, K, R, stream);
+  });
 }
 
 }  // namespace qb200

@@ -1,5 +1,7 @@
 // Internal helpers shared by the translation units of libqlora_b200.so.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -46,12 +48,44 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaS
   return check_launch(what);
 }
 
-// Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16: problem q with its optional LoRA term
-// U[M,R] . V[N,R]^T (R = 0: none) and an optional per-row weight scale row_scale[N] (null: none); every 16-bit operand is of
-// type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16).  bf16 only: state_f16 = 1 reads an fp16 quant state's weights
-// bf16_rn(fp16_rn(LUT[j] * absmax)), out_f16 = 1 writes the bf16-rounded result rounded to fp16.
-int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, int dtype, int state_f16,
-                      int out_f16, cudaStream_t stream);
+// The kernels of an NF4 linear launch, one value per set compiled: the 16-bit operand type T16 and, under bf16 compute, the
+// weights of an fp16 quant state (kStateF16: bf16_rn(fp16_rn(LUT[j] * absmax))) and an fp16 output (kOutF16: the bf16-rounded
+// result rounded to fp16).  fp16 compute reads the same table for an fp16 or fp32 state and has no fp16-output form.
+enum class Nf4Kernels { kBf16, kBf16StateF16, kBf16OutF16, kBf16StateF16OutF16, kF16 };
+
+// A launch's kernels plus out_f32: a 16-bit output widened to fp32 (never with kOutF16).
+struct Nf4Variant {
+  Nf4Kernels kernels;
+  bool out_f32;
+};
+
+// The compile-time parameters of one Nf4Kernels value.
+template <typename T16_, bool kStateF16_, bool kOutF16_>
+struct Nf4Types {
+  using T16 = T16_;
+  static constexpr bool kStateF16 = kStateF16_;
+  static constexpr bool kOutF16 = kOutF16_;
+};
+
+// fn(Nf4Types<...>{}) for the parameters of `k`: the one place the kernel templates are instantiated from a runtime value.
+template <typename Fn>
+auto with_nf4_types(Nf4Kernels k, Fn&& fn) {
+  using BF = __nv_bfloat16;
+  switch (k) {
+    case Nf4Kernels::kBf16StateF16: return fn(Nf4Types<BF, true, false>{});
+    case Nf4Kernels::kBf16OutF16: return fn(Nf4Types<BF, false, true>{});
+    case Nf4Kernels::kBf16StateF16OutF16: return fn(Nf4Types<BF, true, true>{});
+    case Nf4Kernels::kF16: return fn(Nf4Types<__half, false, false>{});
+    case Nf4Kernels::kBf16: break;
+  }
+  return fn(Nf4Types<BF, false, false>{});
+}
+
+// Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16 and a 16-bit output: problem q with its
+// optional LoRA term U[M,R] . V[N,R]^T (R = 0: none) and an optional per-row weight scale row_scale[N] (null: none), run by
+// the skinny kernels of `kernels`.
+int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, Nf4Kernels kernels,
+                      cudaStream_t stream);
 
 // dequantize_4bit(W, state) of problem q as bf16 [N, K] into `out` (32-byte aligned) with the table kernel of nf4_quant.cu —
 // the weights the fused GEMM builds in shared memory, bit for bit (blocks of 64, nested blocks of 256).  Launched with

@@ -514,20 +514,21 @@ _F16_CODE = DTYPE_CODE[torch.float16]
 
 def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None, vs=None, outs=None,
                      out_dtype: Optional[torch.dtype] = None, row_scales=None):
-    """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group`).
+    """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group_ex`, or
+    `qb200_nf4_linear_group_typed` with row scales).
 
     The inputs' dtype (bf16 or fp16) is the compute dtype: U / V / bias are of it too and `out_dtype` is it (the default) or
     fp32 (the result rounded to it, widened); under bf16 compute it may also be fp16 (the bf16-rounded result rounded to
     fp16).  The states share one dtype, which selects the weights: those of `dequantize_4bit(...).to(compute dtype)`.
-    fp16 launches go through `qb200_nf4_linear_group_typed`; their event-log kinds end in `_f16`.  bf16 launches over an fp16
-    state or with an fp16 output go through `qb200_nf4_linear_group_ex`; their kinds end in `_sf16` and / or `_of16`.
+    Event-log kinds end in `_f16` for fp16 compute, and in `_sf16` and / or `_of16` for bf16 compute over an fp16 state or
+    with an fp16 output.
 
     forward  (is_bwd=False): out_p = in_p . W_p^T (+bias_p) + U_p . V_p^T for every problem (the inputs may be one tensor);
                              returns the list of outputs.
     backward (is_bwd=True) : ONE output  sum_p (in_p . W_p + U_p . V_p), accumulated in the kernel; returns it.
     Inputs / U / outputs may be column slices of wider row-major buffers (row pitch passed through).
     row_scales: None, or one fp32 [N] tensor (or None) per problem; W_p is then diag(row_scales[p]) . W_p, the scale folded
-    into the absmax of every NF4 block of the row (`qb200_nf4_linear_group_scaled`).
+    into the absmax of every NF4 block of the row.
     """
     n = len(states)
     assert 1 <= n <= 3 and len(inputs) == n and len(packeds) == n
@@ -548,7 +549,7 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     out_dtype = cdt if out_dtype is None else out_dtype
     out_ok = (cdt, torch.float32, torch.float16) if cdt == torch.bfloat16 else (cdt, torch.float32)
     assert out_dtype in out_ok, f"out_dtype: one of {out_ok}, got {out_dtype}"
-    # bf16 compute over an fp16 state or with an fp16 output: the `_ex` entry point
+    # bf16 compute over an fp16 state or with an fp16 output: the fused kernel at every token count, no row scales
     ex = twice or (cdt == torch.bfloat16 and out_dtype == torch.float16)
     assert not (ex and row_scales is not None), "row scales need a bf16 or fp32 state and a bf16 or fp32 output"
     if outs is None:
@@ -624,19 +625,12 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
             + ("_sf16" if twice else "") + ("_of16" if ex and out_dtype == torch.float16 else ""))
     with torch.cuda.device(dev):
         ev = _event_begin()
-        if ex:
+        if scales is None:
             rc = lib.qb200_nf4_linear_group_ex(int(is_bwd), DTYPE_CODE[cdt], DTYPE_CODE[sdt], n, ct.addressof(probs), r, m, n_out, k_in,
                                                DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
-        elif cdt == torch.float16:
-            rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), _F16_CODE, n, ct.addressof(probs),
-                                                  None if scales is None else ct.addressof(scales), r, m, n_out, k_in,
-                                                  DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
-        elif scales is None:
-            rc = lib.qb200_nf4_linear_group(int(is_bwd), n, ct.addressof(probs), r, m, n_out, k_in,
-                                            0 if out_dtype == torch.float32 else 2, ptr(ws), ws_bytes, stream_ptr(dev))
         else:
-            rc = lib.qb200_nf4_linear_group_scaled(int(is_bwd), n, ct.addressof(probs), ct.addressof(scales), r, m, n_out, k_in,
-                                                   0 if out_dtype == torch.float32 else 2, ptr(ws), ws_bytes, stream_ptr(dev))
+            rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), DTYPE_CODE[cdt], n, ct.addressof(probs), ct.addressof(scales), r, m,
+                                                  n_out, k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
         check(rc, what)
         _event_end(what, m * n, n_out, k_in, ev)
     return outs[0] if is_bwd else outs
