@@ -494,6 +494,17 @@ static int64_t scratch_bytes(int64_t nprob, int64_t M, int64_t N, int64_t K) {
   return M >= scratch_min_m() ? nprob * N * K * 2 : 0;
 }
 
+// The scratch kernel stores a bf16 output by TMA, which needs a 16-byte aligned base and row pitch: true when every output
+// of the call has them (a dX group writes one output), or when the output is fp32 (stored from registers).
+static bool out_tma_aligned(int is_bwd, int nprob, const qb200_nf4_problem* probs, int64_t F, bool out_f32) {
+  if (out_f32) return true;
+  for (int i = 0; i < (is_bwd ? 1 : nprob); ++i) {
+    const int64_t ld = probs[i].ld_out > 0 ? probs[i].ld_out : F;
+    if (reinterpret_cast<uintptr_t>(probs[i].out) % 16 != 0 || ld % 8 != 0) return false;
+  }
+  return true;
+}
+
 template <bool kTrans>
 static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
   sc::Maps maps;
@@ -504,6 +515,7 @@ static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
   for (int i = 0; i < kMaxProb; ++i) {
     if (i >= g.nprob) {
       maps.w[i] = maps.w[0];
+      maps.out[i] = maps.out[0];
       continue;
     }
     // W_p as bf16 [N, K]: box {64, 128} = the K-major forward A tile, {64, 64} = one 64-feature atom of the MN-major dX tile
@@ -511,6 +523,15 @@ static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
     rc = make_map_2d(&maps.w[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, w, uint64_t(g.K), uint64_t(g.N), uint64_t(g.K) * 2, kBlockC,
                      kTrans ? kBlockC : kBlockF, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
+    // Out_p as bf16 [T, F]: box {64 features, 16 tokens} = one 16-token slice of a warpgroup's staging tile (the caller
+    // guarantees a 16-byte aligned base and pitch: out_tma_aligned); fp32 outputs are stored from registers
+    if (p.out_f32) {
+      maps.out[i] = maps.in[i];
+    } else {
+      rc = make_map_2d(&maps.out[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, p.pr[i].out, uint64_t(p.F), uint64_t(p.T),
+                       uint64_t(p.pr[i].ld_out) * 2, 64, sc::kOutBoxT, CU_TENSOR_MAP_SWIZZLE_128B);
+      if (rc) return rc;
+    }
   }
   Strip s;
   rc = plan_strip(p, s);
@@ -582,7 +603,8 @@ static bool nf4_variant(int dtype, int state_dtype, int out_dtype, Nf4Variant& v
 // ---- general entry point: 1..3 problems of one shape in ONE launch, each with an optional row scale; 16-bit operands of
 // type `dtype` (QB200_DTYPE_BF16 or QB200_DTYPE_F16) over a quant state of `state_dtype`, output of `out_dtype` -----------
 // Training token counts (M >= scratch_min_m()) under bf16 compute over a bf16 or fp32 state, with a bf16 or fp32 output and
-// no row-scale array, take the scratch path: `workspace` must then hold scratch_bytes() of 32-byte aligned device memory.  fp16
+// no row-scale array, take the scratch path: `workspace` must then hold scratch_bytes() of 32-byte aligned device memory.  A
+// bf16 output whose base or row pitch is not 16-byte aligned (TMA stores) runs the fused kernel instead.  fp16
 // compute, fp16 states, fp16 outputs and row-scaled launches keep the fused kernel at every token count, as do the four
 // entry points without a workspace (fused_only).
 static int linear_group(int is_bwd, int dtype, int state_dtype, int out_dtype, int nprob, const qb200_nf4_problem* probs,
@@ -620,7 +642,8 @@ static int linear_group(int is_bwd, int dtype, int state_dtype, int out_dtype, i
     }
     return 0;
   }
-  if (!fused_only && v.kernels == Nf4Kernels::kBf16 && !row_scales && M >= gemm::scratch_min_m()) {
+  if (!fused_only && v.kernels == Nf4Kernels::kBf16 && !row_scales && M >= gemm::scratch_min_m() &&
+      gemm::out_tma_aligned(is_bwd, nprob, probs, is_bwd ? K : N, v.out_f32)) {
     const int64_t need = gemm::scratch_bytes(nprob, M, N, K);
     if (workspace == nullptr || workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 32 != 0)
       return set_error(QB200_EINVAL, "nf4_linear: this token count needs a 32-byte aligned bf16 weight scratch of "

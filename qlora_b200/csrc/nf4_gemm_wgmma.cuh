@@ -471,7 +471,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
 // per call instead of once per 128-token unit.  Both operands arrive by TMA and the tensor core sets the pace.
 //
 // Units are 128 features x up to 256 tokens (wgmma m64nNk16, N <= 256, one M=64 half per consumer warpgroup), with the same
-// LoRA step, grouped forms and epilogue as the fused kernel above; the A tile of a step is the same 16 KB K-major (forward)
+// LoRA step, grouped forms and output arithmetic as the fused kernel above; the A tile of a step is the same 16 KB K-major (forward)
 // or MN-major (dX) tile the dequantizers build, loaded from the scratch instead.  Each output element sums the same products
 // in the same order (NF4 steps in order, then the LoRA step) as the fused kernel.
 //
@@ -486,7 +486,11 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
 // Roles (384 threads): warps 0-7 two consumer warpgroups (setmaxnreg 232: 128 accumulators of m64n256) | warps 8-11 the
 // producer warpgroup (setmaxnreg 40), whose first thread issues every TMA.
 // Barriers: full[s] arrive.expect_tx by the producer + TMA complete_tx of the A and activation tiles -> consumers;
-//           empty[s] 8 consumer-warp arrivals once the step's wgmma group has completed -> producer.
+//           empty[s] 8 consumer-warp arrivals once the step's wgmma group has completed -> producer;
+//           named barrier 1 + wg: the 128 threads of consumer warpgroup wg around its output staging tile.
+// Epilogue (bf16 outputs, store_unit_tma): each warpgroup stages its results in its own shared-memory tile and one thread
+// TMA-stores them, so the unit's global writes drain while the warpgroup already issues the next unit's MMAs; fp32 outputs
+// keep store_unit.
 // Programmatic dependent launch: the producer waits (griddepcontrol.wait) before its first load (the scratch is the output
 // of the dequant kernel launched just before), the consumers before their first output store.
 namespace sc {
@@ -494,7 +498,14 @@ constexpr int kUnitT = 256;                                 // max tokens per un
 constexpr int kInSlotBytes = kUnitT * kBlockC * 2;          // 32 KB: one activation block
 constexpr int kStages = 4;                                  // 4 x (16 KB A + 32 KB activations)
 constexpr int kSmemTiles = kStages * (kInSlotBytes + kATileBytes);   // 192 KB
-constexpr int kSmemBytes = kSmemTiles + 1024 + 1024;        // + barriers, + 1 KB alignment of the swizzled tiles
+// Output staging, one tile per consumer warpgroup: 64 features x kOutChunkT tokens of bf16, token rows of 128 B with the
+// 128-byte swizzle of the output map's box.  Four stages leave room for 128-token tiles, so a 256-token unit is staged
+// twice (measured faster in the 7B step than three stages with whole-unit tiles: DESIGN.md 4.1).
+constexpr int kOutChunkT = 128;
+constexpr int kOutBoxT = 16;                                // token rows per TMA store: unit edges are multiples of 16
+constexpr int kOutTileBytes = kOutChunkT * 64 * 2;
+constexpr int kSmemBytes = kSmemTiles + 2 * kOutTileBytes + 1024 + 1024;   // + barriers, + 1 KB alignment of the tiles
+static_assert(kSmemBytes <= 227 * 1024, "scratch kernel exceeds the 227 KB of shared memory of a block");
 constexpr int kConsumerWarps = 8;
 constexpr int kNumThreads = 32 * (kConsumerWarps + 4);      // 384
 constexpr int kConsumerRegs = 232;
@@ -506,6 +517,7 @@ struct Maps {
   CUtensorMap u[kMaxProb];    // LoRA U_p[T, r], box {64, 256}
   CUtensorMap v[kMaxProb];    // LoRA V_p: [F, r] forward, [r, F] dX (as in wg::Maps)
   CUtensorMap w[kMaxProb];    // bf16 W_p[N, K] in the scratch: box {64, 128} forward (K-major A), {64, 64} dX (MN-major A)
+  CUtensorMap out[kMaxProb];  // bf16 Out_p[T, F], pitch ld_out: box {64, 16} (bf16 outputs only)
 };
 
 // A CTA's cursor is a token-row of the strip: below tail0 it is the first row of one of its round units, from tail0 on it
@@ -555,10 +567,60 @@ __device__ __forceinline__ Work decode_work(int a, int end, const Sched& sched, 
   return w;
 }
 
+// Output of warpgroup `wg`'s 64 x kN part of a unit (bf16 outputs) through its staging tile `stage`: the same arithmetic as
+// store_unit (+ bias in fp32, one bf16 rounding), transposed into token rows by stmatrix, then TMA stores of 16-token boxes
+// that cover exactly the unit's tokens [t0, t0 + nt) (TMA clips at T and F).  The warpgroup goes on to its next unit while
+// the stores drain; only the staging tile's next fill waits for them to have read it (wait_group.read by the thread that
+// issued them, then the warpgroup's named barrier).
+template <int kN>
+__device__ __forceinline__ void store_unit_tma(const Work& w, const Params& p, const Maps& maps, int wg, int warp, int lane,
+                                               uint32_t stage, float (&acc)[ptx::kWgmmaWideAcc]) {
+  ptx::grid_dep_wait();   // the output buffer (and bias) may still be in use by an earlier kernel; no-op after the first call
+  if (p.debug & 4) return;
+  const bool leader = (threadIdx.x & 127) == 0;   // issues, commits and waits for the warpgroup's stores
+  const int wq = warp & 3;
+  // thread (wq, lane) holds features f0 + 64 wg + 16 wq + lane / 4 (+ 8): see store_unit
+  const int fa = w.f0 + wg * 64 + wq * 16 + (lane >> 2);
+  const __nv_bfloat16* bias = static_cast<const __nv_bfloat16*>(p.pr[w.prob].bias);
+  const float b0 = bias != nullptr && fa < p.F ? widen(bias[fa]) : 0.0f;
+  const float b1 = bias != nullptr && fa + 8 < p.F ? widen(bias[fa + 8]) : 0.0f;
+  // lane's stmatrix row: matrix m = lane / 8 is features +8 (m & 1) x tokens +8 (m >> 1); row = token lane % 8 of it, whose
+  // 16-byte chunk 2 wq + (m & 1) of the 128-byte token row sits at chunk ^ (token % 8) under the 128-byte swizzle
+  const uint32_t r = uint32_t(lane & 7), m = uint32_t(lane >> 3);
+  const uint32_t row_addr = stage + (8u * (m >> 1) + r) * 128u + (((2u * uint32_t(wq) + (m & 1u)) ^ r) << 4);
+  constexpr int kChunks = (kN + kOutChunkT - 1) / kOutChunkT;
+#pragma unroll
+  for (int c = 0; c < kChunks; ++c) {
+    if (leader) ptx::bulk_wait_group_read<0>();   // the tile's previous stores have read it
+    ptx::bar_sync_warpgroup(1u + uint32_t(wg));
+#pragma unroll
+    for (int jj = 0; jj < kOutChunkT / 16; ++jj) {
+      const int j = c * (kOutChunkT / 8) + 2 * jj;   // the 16 tokens of 8-token groups j, j + 1
+      if (8 * j >= kN) break;
+      ptx::stmatrix_x4_trans(row_addr + uint32_t(jj) * 16u * 128u,
+                             round16x2<__nv_bfloat16>(acc[4 * j + 0] + b0, acc[4 * j + 1] + b0),
+                             round16x2<__nv_bfloat16>(acc[4 * j + 2] + b1, acc[4 * j + 3] + b1),
+                             round16x2<__nv_bfloat16>(acc[4 * j + 4] + b0, acc[4 * j + 5] + b0),
+                             round16x2<__nv_bfloat16>(acc[4 * j + 6] + b1, acc[4 * j + 7] + b1));
+    }
+    ptx::fence_proxy_async_smem();                 // the tile's writes -> visible to the TMA
+    ptx::bar_sync_warpgroup(1u + uint32_t(wg));
+    const int fo = w.f0 + wg * 64;
+    if (leader && fo < p.F) {
+      // rows past nt belong to the next unit (of this or another CTA), or are stale rows of a narrower wgmma N
+      const int n = w.nt - c * kOutChunkT < kOutChunkT ? w.nt - c * kOutChunkT : kOutChunkT;
+      for (int b = 0; b * kOutBoxT < n; ++b)
+        ptx::tma_store_2d(&maps.out[w.prob], stage + uint32_t(b) * (kOutBoxT * 128u), fo, w.t0 + c * kOutChunkT + b * kOutBoxT);
+      ptx::bulk_commit_group();
+    }
+  }
+}
+
 // Consumer warpgroup `wg`: all steps of one unit with wgmma N = kN (>= the unit's tokens), then the output stores.
 template <int kN, bool kTrans>
-__device__ __forceinline__ void consume_unit(const Work& w, const Params& p, const Sched& sched, int wg, int warp, int lane,
-                                             uint32_t smem_base, uint32_t aux, uint32_t& g, float (&acc)[ptx::kWgmmaWideAcc]) {
+__device__ __forceinline__ void consume_unit(const Work& w, const Params& p, const Maps& maps, const Sched& sched, int wg, int warp,
+                                             int lane, uint32_t smem_base, uint32_t aux, uint32_t stage, uint32_t& g,
+                                             float (&acc)[ptx::kWgmmaWideAcc]) {
   auto in_tile = [&](int s) { return smem_base + uint32_t(s) * kInSlotBytes; };
   auto a_tile = [&](int s) { return smem_base + uint32_t(kStages) * kInSlotBytes + uint32_t(s) * kATileBytes; };
   auto full = [&](int s) { return aux + 8u * uint32_t(s); };
@@ -589,7 +651,12 @@ __device__ __forceinline__ void consume_unit(const Work& w, const Params& p, con
   ptx::wgmma_wait<0>(acc);
   __syncwarp();
   if (lane == 0) ptx::mbar_arrive(empty(int((g - 1) % kStages)));
-  store_unit<__nv_bfloat16, kN, false>(w, p, sched, wg, warp, lane, acc);
+  // fp32 outputs (Linear4bit called with fp32 activations) keep the register epilogue: they are off the bf16 training path
+  // and would need twice the staging space
+  if (p.out_f32)
+    store_unit<__nv_bfloat16, kN, false>(w, p, sched, wg, warp, lane, acc);
+  else
+    store_unit_tma<kN>(w, p, maps, wg, warp, lane, stage, acc);
 }
 
 template <bool kTrans>
@@ -599,7 +666,8 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   auto in_tile = [&](int s) { return smem_base + uint32_t(s) * kInSlotBytes; };
   auto a_tile = [&](int s) { return smem_base + uint32_t(kStages) * kInSlotBytes + uint32_t(s) * kATileBytes; };
-  const uint32_t aux = smem_base + uint32_t(kSmemTiles);
+  const uint32_t out_tiles = smem_base + uint32_t(kSmemTiles);   // one output staging tile per consumer warpgroup
+  const uint32_t aux = out_tiles + uint32_t(2 * kOutTileBytes);
   auto full = [&](int s) { return aux + 8u * uint32_t(s); };
   auto empty = [&](int s) { return aux + 8u * uint32_t(kStages + s); };
 
@@ -614,6 +682,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
     for (int i = 0; i < p.nprob; ++i) {
       ptx::tma_prefetch_desc(&maps.in[i]);
       ptx::tma_prefetch_desc(&maps.w[i]);
+      if (!p.out_f32) ptx::tma_prefetch_desc(&maps.out[i]);
       if (has_lora) {
         ptx::tma_prefetch_desc(&maps.u[i]);
         ptx::tma_prefetch_desc(&maps.v[i]);
@@ -663,6 +732,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
     // ===================== consumers: two warpgroups, wgmma + output =====================
     ptx::setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;
+    const uint32_t stage = out_tiles + uint32_t(wg * kOutTileBytes);
     uint32_t g = 0;
     float acc[ptx::kWgmmaWideAcc];
 #pragma unroll
@@ -673,24 +743,25 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
       // N: the unit's tokens rounded up to 16 up to 128, to 32 above
       if (w.nt <= 128) {
         switch (w.nt >> 4) {
-          case 1: consume_unit<16, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 2: consume_unit<32, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 3: consume_unit<48, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 4: consume_unit<64, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 5: consume_unit<80, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 6: consume_unit<96, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 7: consume_unit<112, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          default: consume_unit<128, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 1: consume_unit<16, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 2: consume_unit<32, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 3: consume_unit<48, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 4: consume_unit<64, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 5: consume_unit<80, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 6: consume_unit<96, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 7: consume_unit<112, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          default: consume_unit<128, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
         }
       } else {
         switch ((w.nt + 31) >> 5) {
-          case 5: consume_unit<160, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 6: consume_unit<192, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          case 7: consume_unit<224, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
-          default: consume_unit<256, kTrans>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
+          case 5: consume_unit<160, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 6: consume_unit<192, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          case 7: consume_unit<224, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
+          default: consume_unit<256, kTrans>(w, p, maps, sched, wg, warp, lane, smem_base, aux, stage, g, acc); break;
         }
       }
     }
+    if ((threadIdx.x & 127) == 0) ptx::bulk_wait_group<0>();   // the warpgroup's last output stores are complete
   }
 }
 

@@ -66,6 +66,35 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap
       : "memory");
 }
 
+// Shared -> global tensor store of one box at coordinates {c0, c1}; the box is clipped at the tensor's bounds.  Completion
+// is tracked per thread by bulk async-groups: commit after the stores, then wait_group_read before the shared source is
+// written again, wait_group before the results must be visible.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src_smem, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
+               "r"(src_smem), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kPending) : "memory");
+}
+template <int kPending>
+__device__ __forceinline__ void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kPending) : "memory");
+}
+
+// ---------------------------------------------------------------- shared-memory matrix store, named barrier ----
+// Four 8x8 b16 matrices, transposed: lane l supplies the row address of matrix l / 8, row l % 8; register r_k holds the
+// lane's pair (row l / 4, columns 2 (l % 4) + {0, 1}) of matrix k, which lands in memory row 2 (l % 4) + {0, 1}, column l / 4.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+// bar.sync over the 128 threads of one warpgroup (id 1.. : barrier 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync_warpgroup(uint32_t id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
 // One lane of a CONVERGED warp (elect.sync): the loop around it stays warp-uniform.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
