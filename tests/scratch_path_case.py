@@ -2,6 +2,7 @@
 
 tests/test_gpu_scratch_gemm.py runs it twice, with QB200_SCRATCH_MIN_M forcing the scratch path (bf16 weight copy +
 TMA-fed GEMM) and the fused path, and split-K disabled in both, then compares the two files bit for bit."""
+import itertools
 import os
 import sys
 
@@ -22,13 +23,14 @@ def bits(t):
 
 def main(path):
     out = {}
-    n, k, r = 1152, 768, 16
-    for nested in (True, False):
+    # 1000 x 1088 with r = 24: partial last feature block (forward 104 wide, dX 64), dX contraction tail 40 of 64, and a
+    # LoRA step whose second k16 MMA is half zero-fill
+    for (n, k, r), nested in itertools.product(((1152, 768, 16), (1000, 1088, 24)), (True, False)):
         ps, qss = zip(*[F.quantize_4bit(make_weight(n, k, seed=50 + i), compress_statistics=nested, quant_type="nf4")
                         for i in range(3)])
         ps = [p.t() for p in ps]
         for m in (64, 256, 777, 2048):
-            tag = f"{int(nested)}_{m}"
+            tag = f"{n}x{k}_{int(nested)}_{m}"
             x = make_act(m, k, seed=m)
             dys = [make_act(m, n, seed=m + 1 + i) for i in range(3)]
             us = [make_act(m, r, seed=m + 10 + i) for i in range(3)]

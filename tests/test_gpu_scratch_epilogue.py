@@ -1,7 +1,8 @@
 """The scratch kernel's output epilogue (nf4_gemm_wgmma.cuh, namespace sc): each consumer warpgroup stages its bf16 results
 in shared memory and TMA-stores them in 16-token boxes that cover exactly its unit's tokens.  The stores must land where the
 register epilogue put them: bitwise the fused kernel's outputs at token counts whose units end off 256- and off 32-token
-boundaries, nothing outside the call's [T, F] output of a caller-pitched buffer, and outputs whose base or pitch TMA cannot
+boundaries, nothing outside the call's [T, F] outputs of a caller-pitched buffer (also through the fp32 register epilogue,
+for dX, and for grouped outputs side by side), and outputs whose base or pitch TMA cannot
 address (not 16-byte aligned) run the fused kernel instead."""
 import os
 import subprocess
@@ -58,18 +59,47 @@ def _kernel_names(fn):
 
 
 @pytest.mark.gpu
-def test_scratch_epilogue_writes_only_the_output(tmp_path):
-    """A caller-pitched output: rows >= T and columns >= F of the [T + 64, ld_out] buffer keep their sentinel."""
-    m, n, k, ld = 2000, 4096 + 8, 4096, 4096 + 72
-    F, packed, qs, x, bias = _problem(m, n, k, 210)
-    sentinel = torch.tensor(-12345.0, dtype=torch.bfloat16)
-    buf = torch.full((m + 64, ld), sentinel.item(), dtype=torch.bfloat16, device="cuda")
-    y = F.nf4_linear_group(False, [x], [packed], [qs], biases=[bias], outs=[buf[:m, :n]])[0]
-    assert y.data_ptr() == buf.data_ptr()
-    ref = F.nf4_linear_fwd(x, packed, qs, bias)
-    torch.cuda.synchronize()
-    assert torch.equal(buf[:m, :n], ref)
-    assert bool((buf[:m, n:] == sentinel.item()).all()) and bool((buf[m:] == sentinel.item()).all())
+def test_scratch_epilogue_writes_only_the_output():
+    """Caller-pitched outputs at partial last feature blocks (8, 120 and 64 features wide) and ragged token counts: forward
+    and dX, bf16 (TMA epilogue) and fp32 (register epilogue) outputs, and a grouped forward.  Each [T, F] output is a view of
+    a [T + 64, ld_out] buffer; the grouped forward's outputs sit side by side with 8 sentinel columns after each (every slice
+    base stays 16-byte aligned).  Every output equals the unpitched call's, and every element outside them keeps its
+    sentinel."""
+    import qlora_b200.functional as F
+
+    cases = [(False, torch.bfloat16, 1), (False, torch.float32, 1), (True, torch.bfloat16, 1), (True, torch.float32, 1),
+             (False, torch.bfloat16, 3)]
+    for m, n, k in [(2000, 4104, 4160), (3000, 11000, 1088), (1543, 200, 192)]:
+        ps, qss, biases = [], [], []
+        for i in range(3):
+            _, packed, qs, x, bias = _problem(m, n, k, 210 + 3 * i)
+            ps.append(packed)
+            qss.append(qs)
+            biases.append(bias)
+        dy = make_act(m, n, seed=209)
+        for is_bwd, out_dtype, nprob in cases:
+            what = (m, n, k, "dx" if is_bwd else "fwd", out_dtype, nprob)
+            f_out = k if is_bwd else n
+            assert F._lib.load().qb200_nf4_linear_scratch_size(nprob, m, n, k, int(is_bwd)) == nprob * n * k * 2, what
+            pitch = f_out + 8
+            ld = nprob * pitch + 64
+            sentinel = torch.tensor(-12345.0, dtype=out_dtype).item()
+            buf = torch.full((m + 64, ld), sentinel, dtype=out_dtype, device="cuda")
+            outs = [buf[:m, i * pitch:i * pitch + f_out] for i in range(nprob)]
+            if is_bwd:
+                refs = [F.nf4_linear_bwd_dx(dy, ps[0], qss[0], out_dtype=out_dtype)]   # unpitched
+                ys = [F.nf4_linear_group(True, [dy], ps[:1], qss[:1], outs=outs, out_dtype=out_dtype)]
+            else:
+                refs = F.nf4_linear_group(False, [x] * nprob, ps[:nprob], qss[:nprob], biases=biases[:nprob], out_dtype=out_dtype)
+                ys = F.nf4_linear_group(False, [x] * nprob, ps[:nprob], qss[:nprob], biases=biases[:nprob], outs=outs,
+                                        out_dtype=out_dtype)
+            torch.cuda.synchronize()
+            inside = torch.zeros(buf.shape, dtype=torch.bool, device="cuda")
+            for i, (y, ref) in enumerate(zip(ys, refs)):
+                assert y.data_ptr() == outs[i].data_ptr(), what
+                assert torch.equal(y, ref), (what, i)
+                inside[:m, i * pitch:i * pitch + f_out] = True
+            assert bool((buf[~inside] == sentinel).all()), what
 
 
 @pytest.mark.gpu

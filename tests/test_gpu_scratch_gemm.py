@@ -107,7 +107,8 @@ def test_scratch_grouped_parity(F, nprob, n, k):
 @pytest.mark.gpu
 def test_scratch_and_fused_paths_are_bitwise_equal(tmp_path):
     """The same calls with the threshold forced to each side (split-K off): every output bit equal, at 64, 256, 777 (ragged)
-    and 2048 tokens, single and grouped, forward and dX, with LoRA, bias and an fp32 output."""
+    and 2048 tokens, single and grouped, forward and dX, with LoRA, bias and an fp32 output, at 1152 x 768 (r = 16) and at
+    the ragged 1000 x 1088 (r = 24)."""
     files = {}
     for side, min_m in (("scratch", "17"), ("fused", str(1 << 30))):
         env = dict(os.environ, QB200_SCRATCH_MIN_M=min_m, QB200_SPLITK_MAX_T="0")
@@ -116,7 +117,7 @@ def test_scratch_and_fused_paths_are_bitwise_equal(tmp_path):
                            capture_output=True, text=True, env=env, timeout=900)
         assert r.returncode == 0, r.stderr[-3000:]
     a, b = np.load(files["scratch"]), np.load(files["fused"])
-    assert sorted(a.files) == sorted(b.files) and len(a.files) == 2 * 4 * 9
+    assert sorted(a.files) == sorted(b.files) and len(a.files) == 2 * 2 * 4 * 9
     diff = [name for name in a.files if not np.array_equal(a[name], b[name])]
     assert not diff, diff
 
