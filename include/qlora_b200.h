@@ -201,6 +201,19 @@ int qb200_nf4_linear_group_typed(int is_bwd, int dtype, int nprob, const qb200_n
 int qb200_nf4_linear_group_ex(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int64_t R, int64_t M,
                               int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- grouped form that reuses the bf16 weight copy of an earlier call ------------------------------------------------
+ * qb200_nf4_linear_group_ex with an in / out flag about the workspace (NULL: exactly qb200_nf4_linear_group_ex).  A call
+ * that takes the scratch path (bf16 compute over a bf16 or fp32 state, M >= the scratch threshold, a bf16 or fp32 output)
+ * first writes the bf16 W_p [N, K] of every problem into the workspace, in problem order, then runs the GEMM over them.
+ *   in : nonzero = the workspace already holds those W_p, left there by an earlier call on the same packed weights and quant
+ *        states that reported 1 (e.g. a gradient-checkpoint recompute's forward, reused by the dX launch of the same
+ *        layer).  A call that takes the scratch path then launches only the GEMM; any other call ignores the flag.
+ *   out: 1 when this call left every W_p in the workspace (it took the scratch path), else 0; 0 on error.
+ * A workspace too short or misaligned for the scratch path returns QB200_EINVAL before any launch, whatever the flag says. */
+int qb200_nf4_linear_group_reuse(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int64_t R,
+                                 int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
+                                 int* w_in_workspace, void* stream);
+
 /* U[M,R] = scale * X[M,K] . A[R,K]^T for 1..16 tokens (bf16 in / out, fp32 sum, one rounding): the lora_A projection that
  * feeds qb200_nf4_linear_group's U operand during generation with an unmerged adapter — peft `lora.Linear.forward`'s
  * `lora_A(dropout(x))` (qlora.py:817-834 through PeftModel); replaces a split-K cuBLAS GEMM + reduce per projection.

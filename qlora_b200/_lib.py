@@ -51,6 +51,8 @@ _SIGS = {
     "qb200_nf4_linear_group_typed": ([_i32, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, _vp], _i32),
     "qb200_lora_project_typed": ([_i32, _vp, _i64, _vp, ct.c_float, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
     "qb200_nf4_linear_group_ex": ([_i32, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, _vp], _i32),
+    "qb200_nf4_linear_group_reuse": ([_i32, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, ct.POINTER(_i32), _vp],
+                                     _i32),
 }
 
 

@@ -65,12 +65,17 @@ class MatMul4Bit(torch.autograd.Function):
 
         fused = ctx.io_dtype is not None or (USE_FUSED and B.shape[0] == 1 and F.fused_supported(quant_state, A.dtype))
         cdt = compute_dtype if ctx.io_dtype is not None else A.dtype
+        scratch = None
         if fused:
             b = bias if (bias is None or bias.dtype == cdt) else bias.to(cdt)
-            y = F.nf4_linear_fwd(F.as_compute_2d(A, cdt), B, quant_state, b, out_dtype=F.out_dtype_for(A.dtype, cdt))
-            output = y.view(*A.shape[:-1], quant_state.shape[0])
+            ys, scratch = F.nf4_linear_group(False, [F.as_compute_2d(A, cdt)], [B], [quant_state], None if b is None else [b],
+                                             out_dtype=F.out_dtype_for(A.dtype, cdt), return_scratch=True)
+            output = ys[0].view(*A.shape[:-1], quant_state.shape[0])
         else:
             output = torch.nn.functional.linear(A, _unfused_weight(B, quant_state, A.dtype).t(), bias)
+        kept = F.scratch_to_save(scratch, ctx.needs_input_grad[0])   # a checkpoint recompute's W copy, for the dX launch
+        ctx.save_for_backward(*kept)
+        ctx.kept_scratch = bool(kept)
         if out is not None:
             out.copy_(output)
             output = out
@@ -97,8 +102,9 @@ class MatMul4Bit(torch.autograd.Function):
             grad_bias = grad_output.reshape(-1, grad_output.shape[-1]).sum(0, dtype=ctx.dtype_bias)
         if req_gradA:
             if ctx.fused and (ctx.io_dtype is not None or grad_output.dtype == ctx.cdt):
-                dx = F.nf4_linear_bwd_dx(F.as_compute_2d(grad_output, ctx.cdt), B, ctx.state,
-                                         out_dtype=F.out_dtype_for(ctx.dtype_A, ctx.cdt))
+                scratch = F.saved_scratch(ctx.saved_tensors) if ctx.kept_scratch else None
+                dx = F.nf4_linear_group(True, [F.as_compute_2d(grad_output, ctx.cdt)], [B], [ctx.state],
+                                        out_dtype=F.out_dtype_for(ctx.dtype_A, ctx.cdt), w_scratch=scratch)
                 grad_A = dx.view(*grad_output.shape[:-1], ctx.state.shape[1])
             else:
                 grad_A = torch.matmul(grad_output, _unfused_weight(B, ctx.state, grad_output.dtype).t())

@@ -506,7 +506,7 @@ static bool out_tma_aligned(int is_bwd, int nprob, const qb200_nf4_problem* prob
 }
 
 template <bool kTrans>
-static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
+static int launch_scratch_gemm(const GroupArgs& g, bool w_in_workspace, cudaStream_t stream) {
   sc::Maps maps;
   Params p;
   int rc = fill_launch(g, kTrans, sc::kUnitT, maps, p);
@@ -537,9 +537,13 @@ static int launch_scratch_gemm(const GroupArgs& g, cudaStream_t stream) {
   rc = plan_strip(p, s);
   if (rc) return rc;
   const ScratchPlan& plan = plan_scratch(s.n_fbg, s.t_pad, s.nsteps, num_ctas());
-  for (int i = 0; i < g.nprob; ++i) {
-    rc = launch_dequant_scratch(g.pr[i], g.N, g.K, static_cast<uint8_t*>(g.workspace) + i * w_bytes, stream);
-    if (rc) return rc;
+  // w_in_workspace: an earlier call on the same weights left every W_p there (the checkpoint recompute's copy, read again
+  // by the dX launch).  QB200_DEBUG_FLAGS bit 16 skips the copies too (wrong results by design: their share of the step).
+  if (!w_in_workspace && !(debug_flags() & 16)) {
+    for (int i = 0; i < g.nprob; ++i) {
+      rc = launch_dequant_scratch(g.pr[i], g.N, g.K, static_cast<uint8_t*>(g.workspace) + i * w_bytes, stream);
+      if (rc) return rc;
+    }
   }
   const auto kern = sc::nf4_scratch_gemm_kernel<kTrans>;
   rc = allow_dynamic_smem(reinterpret_cast<const void*>(kern), sc::kSmemBytes);
@@ -606,10 +610,13 @@ static bool nf4_variant(int dtype, int state_dtype, int out_dtype, Nf4Variant& v
 // no row-scale array, take the scratch path: `workspace` must then hold scratch_bytes() of 32-byte aligned device memory.  A
 // bf16 output whose base or row pitch is not 16-byte aligned (TMA stores) runs the fused kernel instead.  fp16
 // compute, fp16 states, fp16 outputs and row-scaled launches keep the fused kernel at every token count, as do the four
-// entry points without a workspace (fused_only).
+// entry points without a workspace (fused_only).  w_in_workspace (null: none) is qb200_nf4_linear_group_reuse's flag: in,
+// the scratch already holds every W_p; out, this call left every W_p there.
 static int linear_group(int is_bwd, int dtype, int state_dtype, int out_dtype, int nprob, const qb200_nf4_problem* probs,
                         const float* const* row_scales, int64_t R, int64_t M, int64_t N, int64_t K, void* workspace,
-                        int64_t workspace_bytes, void* stream, bool fused_only = false) {
+                        int64_t workspace_bytes, void* stream, bool fused_only = false, int* w_in_workspace = nullptr) {
+  const bool reuse = w_in_workspace != nullptr && *w_in_workspace != 0;
+  if (w_in_workspace) *w_in_workspace = 0;
   Nf4Variant v;
   if (!nf4_variant(dtype, state_dtype, out_dtype, v))
     return set_error(QB200_EINVAL, "nf4_linear_group_ex: unsupported (dtype, state_dtype, out_dtype): bf16 compute takes a bf16, fp16 "
@@ -648,7 +655,9 @@ static int linear_group(int is_bwd, int dtype, int state_dtype, int out_dtype, i
     if (workspace == nullptr || workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 32 != 0)
       return set_error(QB200_EINVAL, "nf4_linear: this token count needs a 32-byte aligned bf16 weight scratch of "
                                      "qb200_nf4_linear_scratch_size() bytes in `workspace`");
-    return is_bwd ? gemm::launch_scratch_gemm<true>(g, s) : gemm::launch_scratch_gemm<false>(g, s);
+    rc = is_bwd ? gemm::launch_scratch_gemm<true>(g, reuse, s) : gemm::launch_scratch_gemm<false>(g, reuse, s);
+    if (rc == 0 && w_in_workspace) *w_in_workspace = (reuse || !(gemm::debug_flags() & 16)) ? 1 : 0;
+    return rc;
   }
   return is_bwd ? gemm::launch_gemm<true>(g, s) : gemm::launch_gemm<false>(g, s);
 }
@@ -683,6 +692,13 @@ extern "C" int qb200_nf4_linear_group_ex(int is_bwd, int dtype, int state_dtype,
                                          int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace, int64_t workspace_bytes,
                                          void* stream) {
   return linear_group(is_bwd, dtype, state_dtype, out_dtype, nprob, probs, nullptr, R, M, N, K, workspace, workspace_bytes, stream);
+}
+
+extern "C" int qb200_nf4_linear_group_reuse(int is_bwd, int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs,
+                                            int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* workspace,
+                                            int64_t workspace_bytes, int* w_in_workspace, void* stream) {
+  return linear_group(is_bwd, dtype, state_dtype, out_dtype, nprob, probs, nullptr, R, M, N, K, workspace, workspace_bytes, stream,
+                      false, w_in_workspace);
 }
 
 extern "C" int64_t qb200_nf4_linear_scratch_size(int nprob, int64_t M, int64_t N, int64_t K, int is_bwd) {

@@ -513,8 +513,9 @@ _F16_CODE = DTYPE_CODE[torch.float16]
 
 
 def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None, vs=None, outs=None,
-                     out_dtype: Optional[torch.dtype] = None, row_scales=None):
-    """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group_ex`, or
+                     out_dtype: Optional[torch.dtype] = None, row_scales=None, w_scratch: Optional[Tensor] = None,
+                     return_scratch: bool = False):
+    """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group_reuse`, or
     `qb200_nf4_linear_group_typed` with row scales).
 
     The inputs' dtype (bf16 or fp16) is the compute dtype: U / V / bias are of it too and `out_dtype` is it (the default) or
@@ -529,6 +530,10 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     Inputs / U / outputs may be column slices of wider row-major buffers (row pitch passed through).
     row_scales: None, or one fp32 [N] tensor (or None) per problem; W_p is then diag(row_scales[p]) . W_p, the scale folded
     into the absmax of every NF4 block of the row.
+    Training token counts (the scratch path) dequantize every W_p into a bf16 scratch that the GEMM reads.  return_scratch:
+    also return that scratch, or None when the call left no W_p there: (result, scratch).  w_scratch: a scratch returned by
+    an earlier call on the same packed weights and states, in the same order; a call that takes the scratch path then skips
+    the dequantize launches and reads it.
     """
     n = len(states)
     assert 1 <= n <= 3 and len(inputs) == n and len(packeds) == n
@@ -555,7 +560,7 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     if outs is None:
         outs = [torch.empty((m, f_out), dtype=out_dtype, device=dev) for _ in range(n_outs)]
     if m == 0:
-        return outs[0] if is_bwd else outs
+        return (outs[0] if is_bwd else outs, None) if return_scratch else (outs[0] if is_bwd else outs)
     keep = []  # tensors that must outlive the launch call
     probs = (_lib.Nf4Problem * n)()
 
@@ -613,27 +618,56 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
             scales[i] = sc.data_ptr()
     ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
     # training token counts under bf16 compute (bf16 or fp32 state, bf16 or fp32 output, no row scale): each W is dequantized
-    # once into a bf16 scratch that a TMA-fed GEMM reads; one dequantize launch per problem precedes the GEMM
+    # once into a bf16 scratch that a TMA-fed GEMM reads; one dequantize launch per problem precedes the GEMM, unless the
+    # caller passes back the scratch of an earlier call (w_scratch)
     scratch = (lib.qb200_nf4_linear_scratch_size(n, m, n_out, k_in, int(is_bwd))
                if cdt == torch.bfloat16 and not ex and scales is None else 0)
     ws_bytes = max(ws_bytes, scratch)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
-    if scratch:
-        LAUNCH_COUNTER[0] += n
+    assert w_scratch is None or (scales is None and w_scratch.dtype == torch.uint8 and w_scratch.device == dev)
+    if w_scratch is not None:
+        ws, ws_bytes = w_scratch, w_scratch.numel()
+    else:
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
+    w_in_ws = ct.c_int(int(w_scratch is not None))
     what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
             + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else "")
             + ("_sf16" if twice else "") + ("_of16" if ex and out_dtype == torch.float16 else ""))
     with torch.cuda.device(dev):
         ev = _event_begin()
         if scales is None:
-            rc = lib.qb200_nf4_linear_group_ex(int(is_bwd), DTYPE_CODE[cdt], DTYPE_CODE[sdt], n, ct.addressof(probs), r, m, n_out, k_in,
-                                               DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
+            rc = lib.qb200_nf4_linear_group_reuse(int(is_bwd), DTYPE_CODE[cdt], DTYPE_CODE[sdt], n, ct.addressof(probs), r, m, n_out,
+                                                  k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, ct.byref(w_in_ws), stream_ptr(dev))
         else:
             rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), DTYPE_CODE[cdt], n, ct.addressof(probs), ct.addressof(scales), r, m,
                                                   n_out, k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
         check(rc, what)
         _event_end(what, m * n, n_out, k_in, ev)
-    return outs[0] if is_bwd else outs
+    if w_in_ws.value and w_scratch is None:
+        LAUNCH_COUNTER[0] += n   # the dequantize launches that wrote the scratch
+    res = outs[0] if is_bwd else outs
+    if return_scratch:
+        return res, (ws if w_in_ws.value else None)
+    return res
+
+
+def scratch_to_save(scratch: Optional[Tensor], needs_dx: bool) -> list:
+    """What an autograd forward saves so that its dX launch can reuse the forward's bf16 weight copy (`nf4_linear_group`'s
+    scratch): nothing when the call left none or no dX will run; the copy itself in a forward that runs inside a backward
+    (a gradient-checkpoint recompute, whose dX follows within the same layer's backward); else a one-byte placeholder of its
+    shape, so that a forward outside backward never holds a copy.  Checkpointing requires the original forward and its
+    recompute to save tensors of equal shape, dtype and device, and only the recompute's saved tensors reach the backward
+    (the recompute's ctx is discarded), so the copy has to travel through `save_for_backward`."""
+    if scratch is None or not needs_dx:
+        return []
+    if torch._C._current_graph_task_id() != -1:
+        return [scratch]
+    return [scratch.new_empty(1).expand(scratch.shape)]
+
+
+def saved_scratch(saved) -> Optional[Tensor]:
+    """The weight copy `scratch_to_save` put last among the saved tensors, or None for its placeholder."""
+    t = saved[-1]
+    return t if t.stride(0) == 1 else None
 
 
 def _linear_ex(is_bwd: bool, inp: Tensor, packed: Tensor, quant_state: QuantState, bias: Optional[Tensor] = None,

@@ -166,9 +166,11 @@ class LoraMatMul4Bit(torch.autograd.Function):
         cdt = lora_as[0].dtype
         x2d = F.as_compute_2d(x, cdt)
         xls, us = _project_inputs(x2d, x_loras, lora_as, scaling)
-        ys = F.nf4_linear_group(False, [x2d] * n, packeds, list(states), us=us, vs=[b.contiguous() for b in lora_bs],
-                                out_dtype=F.out_dtype_for(x.dtype, cdt))
-        ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs)
+        ys, scratch = F.nf4_linear_group(False, [x2d] * n, packeds, list(states), us=us, vs=[b.contiguous() for b in lora_bs],
+                                         out_dtype=F.out_dtype_for(x.dtype, cdt), return_scratch=True)
+        kept = F.scratch_to_save(scratch, ctx.needs_input_grad[0])   # a checkpoint recompute's W copies, for the dX launch
+        ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs, *kept)
+        ctx.kept_scratch = bool(kept)
         ctx.adapters = (lora_as, lora_bs)   # the Parameter objects themselves (their .grad buffers, see _adapter_grad)
         ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, x_loras[0] is not None
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
@@ -179,7 +181,9 @@ class LoraMatMul4Bit(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grad_ys):
         n, split = ctx.n, ctx.split
-        xls, us, packeds, lora_as, lora_bs = _split(ctx.saved_tensors, n, 5)
+        saved = ctx.saved_tensors
+        xls, us, packeds, lora_as, lora_bs = _split(saved, n, 5)
+        scratch = F.saved_scratch(saved) if ctx.kept_scratch else None
         need_xl, _, need_a, need_b = _split(ctx.needs_input_grad[4:], n, 4)
         cdt = lora_as[0].dtype
         g2ds = [F.as_compute_2d(g, cdt) for g in grad_ys]
@@ -189,7 +193,8 @@ class LoraMatMul4Bit(torch.autograd.Function):
         grad_xls = [None] * n
         if split:
             if ctx.needs_input_grad[0]:
-                grad_x = F.nf4_linear_group(True, g2ds, packeds, list(ctx.states), out_dtype=out_dtype).view(ctx.x_shape)
+                grad_x = F.nf4_linear_group(True, g2ds, packeds, list(ctx.states), out_dtype=out_dtype,
+                                            w_scratch=scratch).view(ctx.x_shape)
             for i in range(n):
                 if need_xl[i]:
                     shape, dtype = ctx.xl_meta[i]
@@ -197,7 +202,7 @@ class LoraMatMul4Bit(torch.autograd.Function):
         elif ctx.needs_input_grad[0]:
             # dX = sum_p (dY_p . W_p + G_p . A_p): ONE launch, one accumulator — no per-linear dX tensors, no adds
             grad_x = F.nf4_linear_group(True, g2ds, packeds, list(ctx.states), us=gs, vs=[a.contiguous() for a in lora_as],
-                                        out_dtype=out_dtype).view(ctx.x_shape)
+                                        out_dtype=out_dtype, w_scratch=scratch).view(ctx.x_shape)
         pa, pb = ctx.adapters
         if split or n == 1:
             grad_as = [_adapter_grad(pa[i], gs[i].t(), xls[i]) if need_a[i] else None for i in range(n)]
