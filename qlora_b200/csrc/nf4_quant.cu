@@ -450,28 +450,40 @@ __global__ void __launch_bounds__(256) dequantize_nf4_fast_kernel(const uint32_t
   }
 }
 
-// Main path (16-bit output, n % 32 == 0, 32-byte aligned output, power-of-two block sizes): one thread = one 16-byte
-// vector of packed nibbles = 32 values of ONE quant block = 64 B of output.
-//   * the block's 16 possible outputs  T16_rne(LUT[j] * absmax)  are built once per thread as a register product table
+// Main path (16-bit output, n % 32 == 0, 32-byte aligned output, power-of-two block sizes): a 16-byte vector of packed
+// nibbles = 32 values of ONE quant block = 64 B of output; a warp expands kTabVecs runs of 32 consecutive vectors per
+// iteration, one vector per lane per run.
+//   * the block's 16 possible outputs  T16_rne(LUT[j] * absmax)  are built once per vector as a register product table
 //     (nf4_table.cuh: 32 instructions per 32 values) and every nibble is resolved with PRMT byte permutes — 2 per value,
 //     no shared-memory look-up, multiply or convert per value (the LUT-in-shared-memory kernel above issues 9.4
 //     instructions per value and stalls on the shared-memory queue: ncu issue-active 61-68 %, mio_throttle 3.3);
-//   * loads are 512 contiguous bytes per warp instruction, stores two 256-bit st.global per thread: every 32-byte sector
-//     is written by exactly one instruction;
-//   * persistent grid (4 CTAs per SM) with the next vector + its absmax statistics prefetched before the current one is
-//     expanded, so loads, look-ups and stores of consecutive iterations overlap.
+//   * loads are 512 contiguous bytes per warp instruction.  A run's 2 KB of output goes through a per-warp shared-memory
+//     stage, so each of its four 16-byte warp stores writes 512 contiguous bytes (4 whole lines).  Storing each lane's
+//     64 B straight from registers writes 16 B at a 64 B stride per instruction (16 lines, every sector half-written) and
+//     ran at 1.25-1.39 TB/s against 2.16-2.50 TB/s for the same loads with a contiguous store mapping
+//     (tools/stream_perf.py, H100 80GB HBM3 at 700 W; this kernel: 2.44-2.66 TB/s).  The stage slot of a lane's k-th 16 B is rotated by lane / 2, which keeps both the
+//     writes (64 B per lane) and the reads (16 B per lane) free of bank conflicts;
+//   * kTabVecs runs in flight per thread, the next iteration's vectors + absmax statistics prefetched before the current
+//     ones are expanded; the grid is capped at kTabCtasPerSm CTAs per SM (about two waves at the registers this kernel
+//     takes) and a grid-stride loop takes the rest.  Two runs per thread and the two-wave grid measured 5-10 % above one
+//     run and a persistent one-wave grid; a second vector in flight without the stage did not help (1.1-1.2 TB/s).
 // kPdl: the bf16 weight copy of the scratch GEMM path (launch_dequant_scratch), launched with programmatic stream
 // serialization: it lets the GEMM queued behind it start its prologue at once and issues its first loads (the frozen
 // quant state) before it waits for the previous kernel, whose reads of a recycled scratch buffer must end before any store.
+constexpr int kTabWarps = 8;        // warps per CTA: 256 threads, one s_code entry each
+constexpr int kTabVecs = 2;         // runs of 32 vectors per warp and iteration
+constexpr int kTabCtasPerSm = 8;
 template <typename T16, bool NESTED, bool kPdl = false>
-__global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __restrict__ packed, const float* __restrict__ absmax,
-                                                                 const uint8_t* __restrict__ absmax_u8,
-                                                                 const float* __restrict__ code256,
-                                                                 const float* __restrict__ absmax2,
-                                                                 const float* __restrict__ offset_ptr, uint32_t nvec,
-                                                                 int bs_shift /* log2(blocksize / 32) */, int bs2_shift,
-                                                                 uint8_t* __restrict__ out) {
+__global__ void __launch_bounds__(32 * kTabWarps) dequantize_nf4_tab_kernel(const uint4* __restrict__ packed,
+                                                                            const float* __restrict__ absmax,
+                                                                            const uint8_t* __restrict__ absmax_u8,
+                                                                            const float* __restrict__ code256,
+                                                                            const float* __restrict__ absmax2,
+                                                                            const float* __restrict__ offset_ptr, uint32_t nvec,
+                                                                            int bs_shift /* log2(blocksize / 32) */, int bs2_shift,
+                                                                            uint8_t* __restrict__ out) {
   __shared__ float s_code[256];
+  __shared__ uint4 s_stage[kTabWarps][128];   // one run's output per warp: 32 vectors x 4 16-byte chunks
   float offset = 0.0f;
   if (NESTED) {
     s_code[threadIdx.x] = code256[threadIdx.x];
@@ -479,34 +491,68 @@ __global__ void __launch_bounds__(256) dequantize_nf4_tab_kernel(const uint4* __
     __syncthreads();
   }
   if constexpr (kPdl) ptx::grid_dep_launch();
-  const uint32_t stride = gridDim.x * blockDim.x;
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  uint4 w_next;
-  uint32_t code_next = 0;
-  float scale_next;
-  auto fetch = [&](uint32_t v) {
-    v = v < nvec ? v : nvec - 1;                       // clamped: the prefetch past the end re-reads the last vector
-    w_next = __ldg(packed + v);
-    const uint32_t b = v >> bs_shift;
-    if (NESTED) {
-      code_next = __ldg(absmax_u8 + b);
-      scale_next = __ldg(absmax2 + (b >> bs2_shift));
-    } else {
-      scale_next = __ldg(absmax + b);
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr uint32_t kSpan = 32 * kTabVecs;   // vectors per warp and iteration
+  const uint32_t stride = gridDim.x * kTabWarps * kSpan;
+  uint32_t base = (blockIdx.x * kTabWarps + warp) * kSpan;
+  uint4 w_next[kTabVecs];
+  uint32_t code_next[kTabVecs];
+  float scale_next[kTabVecs];
+  auto fetch = [&](uint32_t b0) {
+#pragma unroll
+    for (int u = 0; u < kTabVecs; ++u) {
+      uint32_t v = b0 + u * 32 + lane;
+      v = v < nvec ? v : nvec - 1;                       // clamped: the prefetch past the end re-reads the last vector
+      w_next[u] = __ldg(packed + v);
+      const uint32_t b = v >> bs_shift;
+      code_next[u] = 0;
+      if (NESTED) {
+        code_next[u] = __ldg(absmax_u8 + b);
+        scale_next[u] = __ldg(absmax2 + (b >> bs2_shift));
+      } else {
+        scale_next[u] = __ldg(absmax + b);
+      }
     }
   };
-  fetch(i);
-  if constexpr (kPdl) ptx::grid_dep_wait();
-  for (; i < nvec; i += stride) {
-    const uint4 w = w_next;
-    const float am = NESTED ? nested_absmax(s_code[code_next], scale_next, offset) : scale_next;
-    fetch(i + stride);
-    Nf4Table tab;
-    build_table<T16>(am, tab);
-    uint8_t* dst = out + (uint64_t(i) << 6);
-    ptx::st_global_32B(dst, dequant_word(w.x, tab), dequant_word(w.y, tab));
-    ptx::st_global_32B(dst + 32, dequant_word(w.z, tab), dequant_word(w.w, tab));
+  fetch(base);
+  if constexpr (kPdl) ptx::grid_dep_wait();           // no global store before this point
+  uint4* out16 = reinterpret_cast<uint4*>(out);
+  for (; base < nvec; base += stride) {               // warp-uniform: the __syncwarp()s below see the whole warp
+    uint4 w[kTabVecs];
+    float am[kTabVecs];
+#pragma unroll
+    for (int u = 0; u < kTabVecs; ++u) {
+      w[u] = w_next[u];
+      am[u] = NESTED ? nested_absmax(s_code[code_next[u]], scale_next[u], offset) : scale_next[u];
+    }
+    fetch(base + stride);
+#pragma unroll
+    for (int u = 0; u < kTabVecs; ++u) {
+      const uint32_t v0 = base + u * 32;              // first vector of the run
+      Nf4Table tab;
+      build_table<T16>(am[u], tab);
+      const uint4 o[4] = {dequant_word(w[u].x, tab), dequant_word(w[u].y, tab), dequant_word(w[u].z, tab),
+                          dequant_word(w[u].w, tab)};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) s_stage[warp][4 * lane + ((k + (lane >> 1)) & 3)] = o[k];
+      __syncwarp();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {                   // chunk c of the run = 16-byte piece c % 4 of vector v0 + c / 4
+        const uint32_t c = 32 * j + lane, src = c >> 2;
+        const uint4 val = s_stage[warp][4 * src + (((c & 3) + (src >> 1)) & 3)];
+        if (v0 + src < nvec) out16[uint64_t(v0) * 4 + c] = val;
+      }
+      __syncwarp();                                   // the stage is rewritten by the next run
+    }
   }
+}
+
+// CTAs of dequantize_nf4_tab_kernel for nvec vectors: kTabVecs runs of 32 vectors per warp, at most kTabCtasPerSm CTAs
+// per SM (the grid-stride loop takes the rest)
+static unsigned tab_grid(uint32_t nvec) {
+  const int64_t per_cta = int64_t(kTabWarps) * 32 * kTabVecs;
+  const int64_t tb = (int64_t(nvec) + per_cta - 1) / per_cta, tb_max = int64_t(device_sm_count()) * kTabCtasPerSm;
+  return unsigned(tb < tb_max ? tb : tb_max);
 }
 
 // QB200_DEQUANT_LUT=1 keeps the shared-memory-LUT kernels for every shape (A/B measurements, tests of that path)
@@ -535,12 +581,9 @@ static int launch_dequantize_nf4(const uint8_t* packed, const float* absmax, con
       if (n % 32 == 0 && reinterpret_cast<uintptr_t>(out) % 32 == 0 && reinterpret_cast<uintptr_t>(packed) % 16 == 0 &&
           !dequant_lut_path()) {
         const uint32_t nvec = uint32_t(n / 32);
-        int64_t tb = (int64_t(nvec) + threads - 1) / threads;
-        const int64_t tb_max = int64_t(device_sm_count()) * 4;   // persistent grid: 4 CTAs per SM
-        if (tb > tb_max) tb = tb_max;
         const auto kern = nested ? dequantize_nf4_tab_kernel<T, true> : dequantize_nf4_tab_kernel<T, false>;
-        kern<<<(unsigned)tb, threads, 0, stream>>>(reinterpret_cast<const uint4*>(packed), absmax, absmax_u8, code256, absmax2, offset,
-                                                   nvec, bs_shift - 2, bs2_shift, reinterpret_cast<uint8_t*>(out));
+        kern<<<tab_grid(nvec), threads, 0, stream>>>(reinterpret_cast<const uint4*>(packed), absmax, absmax_u8, code256, absmax2,
+                                                     offset, nvec, bs_shift - 2, bs2_shift, reinterpret_cast<uint8_t*>(out));
         return check_launch("dequantize_nf4");
       }
       const int64_t fb_max = int64_t(device_sm_count()) * 16;
@@ -563,12 +606,9 @@ static bool valid_blocksize(int bs) { return bs >= 64 && bs <= 4096 && (bs & (bs
 
 int launch_dequant_scratch(const qb200_nf4_problem& q, int64_t N, int64_t K, void* out, cudaStream_t stream) {
   const uint32_t nvec = uint32_t(N * K / 32);   // 32 values (16 packed bytes) per vector; blocks of 64, nested blocks of 256
-  int64_t tb = (int64_t(nvec) + 255) / 256;
-  const int64_t tb_max = int64_t(device_sm_count()) * 4;
-  if (tb > tb_max) tb = tb_max;
   using BF = __nv_bfloat16;
   const auto kern = q.absmax_u8 != nullptr ? dequantize_nf4_tab_kernel<BF, true, true> : dequantize_nf4_tab_kernel<BF, false, true>;
-  return launch_pdl(kern, unsigned(tb), 256, 0, stream, "dequantize_nf4_scratch", reinterpret_cast<const uint4*>(q.packed),
+  return launch_pdl(kern, tab_grid(nvec), 256, 0, stream, "dequantize_nf4_scratch", reinterpret_cast<const uint4*>(q.packed),
                     q.absmax_f32, q.absmax_u8, q.code256, q.absmax2, q.offset, nvec, 1, 8, static_cast<uint8_t*>(out));
 }
 

@@ -319,12 +319,5 @@ __device__ __forceinline__ uint32_t cvt_f16x2(float lo_f, float hi_f) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi_f), "f"(lo_f));
   return d;
 }
-// 32 bytes (one full sector) as two 16-byte global stores (the widest store sm_90 has)
-__device__ __forceinline__ void st_global_32B(void* p, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};\n\tst.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(p), "r"(a.x), "r"(a.y),
-               "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
-}
-
 }  // namespace ptx
 }  // namespace qb200

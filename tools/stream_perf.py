@@ -5,7 +5,10 @@ Every case is a CUDA graph of `reps` launches that rotate over enough distinct w
 (no flush kernels inside the timed region; every launch reads its operands from HBM), timed with CUDA events; the
 per-launch figure is graph time / reps, so it includes the back-to-back launch gap a decode loop would see.
 
-  python tools/stream_perf.py [--lib path/to/libqlora_b200.so] [--what skinny,dequant,quant] [--out file.jsonl]
+  python tools/stream_perf.py [--lib path/to/libqlora_b200.so] [--what skinny,dequant,quant,ceiling] [--out file.jsonl]
+
+`ceiling` (with `dequant`) adds a device-to-device copy_ and a write-only fill_ at each dequantize's byte count: the
+rates the same card reaches for pure streaming.  The first line names the card and its power limit.
   python tools/stream_perf.py --ncu       # one launch of each kernel after a flush, for `ncu --set full`
 """
 import argparse
@@ -82,6 +85,40 @@ def copies_for(nbytes):
     return max(2, -(-int(1.5 * L2_BYTES) // nbytes))
 
 
+def card():
+    """Name and power limit of the card the numbers are measured on."""
+    import subprocess
+
+    d = {"gpu": torch.cuda.get_device_name()}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader",
+                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30)
+        d["power_limit"], d["max_sm_clock"] = (v.strip() for v in q.stdout.strip().split(","))
+    except Exception as e:   # no nvidia-smi: the name alone
+        d["power_limit"] = f"unknown ({type(e).__name__})"
+    return d
+
+
+def ceilings(n, k, nm, alg):
+    """Two HBM ceilings at the byte count `alg` of a dequantize: a device-to-device copy_ (alg / 2 read + alg / 2 written)
+    and a write-only fill_ of alg bytes."""
+    half = alg // 2
+    nc = copies_for(alg)
+    src = [torch.empty(half, dtype=torch.uint8, device="cuda").fill_(1) for _ in range(nc)]
+    dst = [torch.empty(half, dtype=torch.uint8, device="cuda") for _ in range(nc)]
+    med, best = graph_time_us([(lambda s=s, d=d: d.copy_(s)) for s, d in zip(src, dst)], reps=4 * nc)
+    emit({"tag": "copy_ceiling_" + nm, "n": n, "k": k, "us": round(med, 2), "us_best": round(best, 2),
+          "GBps": round(2 * half / med / 1e3, 1), "frac_hbm": round(2 * half / med / 1e3 / PEAK, 3), "copies": nc})
+    del src, dst
+    buf = [torch.empty(alg, dtype=torch.uint8, device="cuda") for _ in range(nc)]
+    med, best = graph_time_us([(lambda b=b: b.fill_(7)) for b in buf], reps=4 * nc)
+    emit({"tag": "fill_ceiling_" + nm, "n": n, "k": k, "us": round(med, 2), "us_best": round(best, 2),
+          "GBps": round(alg / med / 1e3, 1), "frac_hbm": round(alg / med / 1e3 / PEAK, 3), "copies": nc})
+    del buf
+
+
+if not args.ncu:
+    emit({"tag": "card", **card()})
 flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")
 
 for n, k in SHAPES:
@@ -126,6 +163,8 @@ for n, k in SHAPES:
             emit({"tag": "dequant_" + nm, "n": n, "k": k, "us": round(med, 2), "us_best": round(best, 2),
                   "GBps": round(alg / med / 1e3, 1), "frac_hbm": round(alg / med / 1e3 / PEAK, 3), "copies": nc})
             del ins, outs
+            if "ceiling" in WHAT:
+                ceilings(n, k, nm, alg)
 
     if "quant" in WHAT and (n, k) != (4096, 11008):
         alg = n * k * 2 + n * k // 2 + (n * k // 64) * 4
