@@ -73,6 +73,7 @@ class AdamW(torch.optim.Optimizer):
         self._paged: dict = {}       # id(param) -> (_ManagedBuffer, _ManagedBuffer); owners of the unified memory
         self._step_dev = None        # capturable: device float32 scalar, shared by every parameter
         self._flat = None            # step_flat: (m, v) over the whole flat parameter buffer
+        self._flat_offsets = None    # step_flat: offset of every parameter (param_groups order) in the flat buffer
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
 
     def _new_moments(self, p):
@@ -94,6 +95,7 @@ class AdamW(torch.optim.Optimizer):
         # fp32 moments from the file itself.  Paged optimizers give them fresh unified-memory homes; a pointer is never
         # adopted from the file.
         self._paged.clear()
+        self._flat = None   # a later step_flat rebuilds its flat moments from the loaded per-parameter slices
         saved_groups = state_dict["param_groups"]
         id_to_param = {}
         for g_saved, g in zip(saved_groups, self.param_groups):
@@ -170,8 +172,9 @@ class AdamW(torch.optim.Optimizer):
     def step_flat(self, flat_param: torch.Tensor, flat_grad: torch.Tensor, grad_scale: torch.Tensor | None = None):
         """ONE launch for ALL parameters when they (and their gradients) are views into two flat buffers of identical layout
         (harness/dp.py keeps the LoRA adapters that way): `flat_param[i]` is updated from `flat_grad[i]` with one pair of
-        flat fp32 moments (paged when `is_paged`).  Needs `capturable=True`; every parameter of the optimizer must live in
-        `flat_param` and share one hyper-parameter group."""
+        flat fp32 moments (paged when `is_paged`).  Needs `capturable=True`; every parameter of the optimizer must be a view
+        into `flat_param` and share one hyper-parameter group.  `state_dict()` publishes the flat moments as per-parameter
+        `state1` / `state2` slices; moments loaded by `load_state_dict` are copied into the flat ones by the next call."""
         if not self.capturable:
             raise ValueError("step_flat needs capturable=True")
         if len(self.param_groups) != 1:
@@ -184,8 +187,8 @@ class AdamW(torch.optim.Optimizer):
         total = sum(p.numel() for p in group["params"])
         if total != flat_param.numel():
             raise ValueError("the flat buffer does not cover exactly the optimizer's parameters")
-        key = "_flat"
-        if not hasattr(self, key) or getattr(self, key) is None:
+        if self._flat is None:
+            self._flat_offsets = self._offsets_in(flat_param, group["params"])
             class _P:   # stand-in carrying numel / device for _new_moments
                 pass
             proxy = _P()
@@ -193,6 +196,12 @@ class AdamW(torch.optim.Optimizer):
             proxy.device = flat_param.device
             self._flat_key = proxy
             m, v = self._new_moments(proxy)
+            for p, off in zip(group["params"], self._flat_offsets):   # moments from load_state_dict (or per-parameter steps)
+                st = self.state.pop(p, None)
+                if st and "state1" in st:
+                    m[off:off + p.numel()].copy_(st["state1"].reshape(-1))
+                    v[off:off + p.numel()].copy_(st["state2"].reshape(-1))
+                self._paged.pop(id(p), None)
             self._flat = (m, v)
         m, v = self._flat
         b1, b2 = group["betas"]
@@ -208,13 +217,36 @@ class AdamW(torch.optim.Optimizer):
                                                         ptr(self._step_dev), ptr(grad_scale), stream_ptr(flat_param.device)),
                   "adamw32bit_step_dev")
 
+    @staticmethod
+    def _offsets_in(flat: torch.Tensor, params) -> list:
+        """Element offset of every parameter in `flat`; each must be a contiguous view into it, and together they cover it."""
+        offs, base, es = [], flat.data_ptr(), flat.element_size()
+        for p in params:
+            off, rem = divmod(p.data_ptr() - base, es)
+            if rem or off < 0 or off + p.numel() > flat.numel() or not p.is_contiguous() or p.dtype != flat.dtype:
+                raise ValueError("step_flat: every parameter must be a contiguous view into the flat parameter buffer")
+            offs.append(off)
+        end = 0
+        for off, n in sorted(zip(offs, (p.numel() for p in params))):
+            if off != end:
+                raise ValueError("step_flat: the parameters overlap or leave a gap in the flat parameter buffer")
+            end = off + n
+        return offs
+
     def state_dict(self):
+        t = None
         if self.capturable and self._step_dev is not None:   # publish the device-side count in the per-parameter `step`s
             t = float(self._step_dev.item())
             for st in self.state.values():
                 if "step" in st:
                     st["step"] = torch.tensor(t, dtype=torch.float32)
-        return super().state_dict()
+        sd = super().state_dict()
+        if self._flat is not None:   # step_flat's moments, one slice per parameter (views: torch.save writes the buffer once)
+            m, v = self._flat
+            for i, (p, off) in enumerate(zip(self.param_groups[0]["params"], self._flat_offsets)):
+                sd["state"][i] = {"step": torch.tensor(t, dtype=torch.float32), "state1": m[off:off + p.numel()],
+                                  "state2": v[off:off + p.numel()]}
+        return sd
 
 
 class AdamW32bit(AdamW):

@@ -1,5 +1,6 @@
 """GPU tests of the bench harness (caller-side scaffolding): fused RoPE / SwiGLU kernels vs their torch formulations,
-and one tiny Llama-QLoRA training step (fused kernel + fused LoRA step + checkpointing) vs the all-unfused variant."""
+one tiny Llama-QLoRA training step (fused kernel + fused LoRA step + checkpointing) vs the all-unfused variant, and the
+harness kernels element by element against float64 (the seeded dropout bit for bit)."""
 import pytest
 import torch
 
@@ -164,3 +165,174 @@ def test_add_rmsnorm_matches_unfused(H, d):
     assert torch.equal(s, s2) and torch.equal(y, y2)
     for a, b in ((x.grad, x2.grad), (dl.grad, d2.grad)):
         assert ((a.float() - b.float()).norm() / b.float().norm()).item() < 4e-3   # one rounding instead of two
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Element-wise checks against float64 computed from the same bf16 inputs.  The bound of every element is one bf16 ulp of
+# the float64 result plus the kernel's fp32 roundings, scaled by the magnitudes of the terms they act on (`mag`): where a
+# backward subtracts nearly equal terms, the fp32 error of those terms can exceed an ulp of the small difference.
+# ---------------------------------------------------------------------------------------------------------------------
+def _bf16_ulp(v: torch.Tensor) -> torch.Tensor:
+    """Spacing of bf16 values at |v| (float64; 0 where v is 0)."""
+    _, e = torch.frexp(v.abs())
+    return torch.where(v == 0, torch.zeros_like(v), torch.ldexp(torch.ones_like(v), e - 8))
+
+
+def _assert_elementwise(got, ref, mag, fp32_ulps, what):
+    got = got.detach().double().cpu()
+    tol = _bf16_ulp(ref) + fp32_ulps * 2.0 ** -24 * mag
+    bad = (got - ref).abs() > tol
+    assert not bad.any(), (f"{what}: {int(bad.sum())} of {bad.numel()} elements off, first at {bad.nonzero()[0].tolist()}: "
+                           f"{got[bad][0].item()} vs {ref[bad][0].item()} (tol {tol[bad][0].item():.3e})")
+
+
+def _f64(t):
+    return t.detach().double().cpu()
+
+
+@pytest.mark.parametrize("n", [4096, 132 * 16 * 256 * 8 + 8 * 4099])   # the second runs past the kernel's grid-stride cap
+def test_seeded_dropout_is_bit_exact(H, n):
+    """The mask and scale of the seeded dropout, forward and backward, against tests/step_reference.py's restatement of the
+    kernel's hash."""
+    import step_reference as R
+    from harness import fused_ops
+
+    torch.manual_seed(11)
+    x = torch.randn(n, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    gy = torch.randn(n, device="cuda").to(torch.bfloat16)
+    for p in (0.0, 0.1, 0.5):
+        scale = torch.tensor(1.0) / (1.0 - torch.tensor(p, dtype=torch.float32))   # the kernel's fp32 1 / (1 - p)
+        for seed, salt in ((1, 1), (2, 1), (1, 2), (123456789, 77)):
+            seed_dev = torch.tensor(seed, device="cuda", dtype=torch.int64)
+            keep = torch.from_numpy(R.dropout_keep(n, p, seed, salt))
+            x.grad = None
+            y = fused_ops.seeded_dropout(x, p, seed_dev, salt)
+            y.backward(gy)
+            for out, src in ((y, x), (x.grad, gy)):
+                want = torch.where(keep, (src.detach().float().cpu() * scale).to(torch.bfloat16), torch.zeros((), dtype=torch.bfloat16))
+                assert torch.equal(out.detach().cpu(), want), (p, seed, salt)
+            if p == 0.0:
+                assert torch.equal(y, x)
+
+
+def test_rope_tables_match_float64(H):
+    """cos and sign-folded sin, [seq, 1, d] bf16: within one bf16 ulp of float64, plus the fp32 rounding of the angle
+    (position x inverse frequency in fp32, as HF computes it)."""
+    s, d, theta = 2048, 128, 10000.0
+    cos, sin = H._rope_tables(s, d, theta, "cuda")
+    assert cos.shape == (s, 1, d) and sin.shape == (s, 1, d)
+    inv = 1.0 / theta ** (torch.arange(0, d, 2, dtype=torch.float64) / d)
+    ang = torch.outer(torch.arange(s, dtype=torch.float64), inv)
+    slack = 2.0 ** -22 * ang.repeat(1, 2)   # the fp32 angle: |error| <= ~2 ulp of it
+    for got, want in ((cos, torch.cat((ang.cos(), ang.cos()), -1)), (sin, torch.cat((-ang.sin(), ang.sin()), -1))):
+        assert ((_f64(got[:, 0]) - want).abs() <= _bf16_ulp(want) + slack).all()
+
+
+def _rope64(x, cos, sin):
+    half = x.shape[-1] // 2
+    return x * cos + torch.cat((x[..., half:], x[..., :half]), -1) * sin
+
+
+@pytest.mark.parametrize("d", [64, 128])
+def test_rope_matches_float64(H, d):
+    """Forward and backward (the kernel with sign -1) at batch 3 with more q heads than k heads (grouped-query attention),
+    every element within one bf16 ulp of float64 from the same bf16 inputs and tables."""
+    from harness import fused_ops
+
+    torch.manual_seed(d)
+    b, s, hq, hk = 3, 97, 8, 2
+    cos, sin = H._rope_tables(s, d, 10000.0, "cuda")
+    q = torch.randn(b, s, hq, d, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    k = torch.randn(b, s, hk, d, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    gq, gk = torch.randn_like(q), torch.randn_like(k)
+    qo, ko = fused_ops.rope_qk(q, k, cos, sin)
+    torch.autograd.backward([qo, ko], [gq, gk])
+    c64, s64 = _f64(cos), _f64(sin)
+    for x, g, out in ((q, gq, qo), (k, gk, ko)):
+        x64 = _f64(x).requires_grad_(True)
+        y64 = _rope64(x64, c64, s64)
+        y64.backward(_f64(g))
+        mag = _rope64(x64.detach().abs(), c64.abs(), s64.abs())
+        _assert_elementwise(out, y64.detach(), mag, 4, f"rope fwd h={x.shape[2]}")
+        gmag = _rope64(_f64(g).abs(), c64.abs(), s64.abs())   # the transpose mixes the same pairs
+        _assert_elementwise(x.grad, x64.grad, gmag, 4, f"rope bwd h={x.shape[2]}")
+
+
+def _rms64(x, w, eps):
+    rstd = torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps)
+    return x * rstd * w, rstd
+
+
+def _rms_bwd_mag(x, w, g, rstd):
+    """Magnitudes of the terms of dx = rstd (g w - x c), c = rstd^2 mean(g w x): what the fp32 roundings act on."""
+    cmag = rstd * rstd * (g * w * x).abs().mean(-1, keepdim=True)
+    return rstd * ((g * w).abs() + x.abs() * cmag)
+
+
+NORM_DIMS = [2048, 2056, 4096, 4104, 8192, 8200]   # each side of the register-tile (2/4/8 vectors) and two-pass boundaries
+
+
+@pytest.mark.parametrize("d", NORM_DIMS)
+def test_rmsnorm_matches_float64(H, d):
+    from harness import fused_ops
+
+    torch.manual_seed(d)
+    x = (torch.randn(3, 67, d, device="cuda") * 2).to(torch.bfloat16).requires_grad_(True)   # 201 rows
+    w = (1 + 0.1 * torch.randn(d, device="cuda")).float()
+    gy = torch.randn_like(x)
+    y = fused_ops.rmsnorm(x, w, 1e-5)
+    y.backward(gy)
+    x64 = _f64(x).requires_grad_(True)
+    w64, g64 = _f64(w), _f64(gy)
+    y64, rstd = _rms64(x64, w64, 1e-5)
+    y64.backward(g64)
+    _assert_elementwise(y, y64.detach(), y64.detach().abs(), d / 4, f"rmsnorm fwd d={d}")
+    _assert_elementwise(x.grad, x64.grad, _rms_bwd_mag(x64.detach(), w64, g64, rstd.detach()), d / 4, f"rmsnorm bwd d={d}")
+
+
+@pytest.mark.parametrize("d", NORM_DIMS)
+def test_add_rmsnorm_matches_float64(H, d):
+    """The residual sum is torch's bf16 `x + delta` exactly; the norm of it and both input gradients (the residual-path
+    gradient plus the norm's backward) within the element bound of float64."""
+    from harness import fused_ops
+
+    torch.manual_seed(d + 1)
+    x = (torch.randn(3, 67, d, device="cuda") * 2).to(torch.bfloat16).requires_grad_(True)
+    dl = torch.randn(3, 67, d, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    w = (1 + 0.1 * torch.randn(d, device="cuda")).float()
+    if d > 8192:   # one CTA holds the row in registers: 8192 is the widest row the fused form takes
+        with pytest.raises(RuntimeError, match="failed"):
+            fused_ops.add_rmsnorm(x, dl, w, 1e-5)
+        return
+    g_s, g_y = torch.randn_like(x), torch.randn_like(x)
+    s, y = fused_ops.add_rmsnorm(x, dl, w, 1e-5)
+    torch.autograd.backward([s, y], [g_s, g_y])
+    assert torch.equal(s.cpu(), (x.detach().float() + dl.detach().float()).to(torch.bfloat16).cpu())
+    s64 = _f64(s).requires_grad_(True)
+    w64, gs64, gy64 = _f64(w), _f64(g_s), _f64(g_y)
+    y64, rstd = _rms64(s64, w64, 1e-5)
+    y64.backward(gy64)
+    _assert_elementwise(y, y64.detach(), y64.detach().abs(), d / 4, f"add_rmsnorm fwd d={d}")
+    want = gs64 + s64.grad
+    mag = gs64.abs() + _rms_bwd_mag(s64.detach(), w64, gy64, rstd.detach())
+    for grad in (x.grad, dl.grad):
+        _assert_elementwise(grad, want, mag, d / 4, f"add_rmsnorm bwd d={d}")
+
+
+def test_swiglu_backward_matches_float64(H):
+    """d_gate = dy u s (1 + g (1 - s)) and d_up = dy g s, s = sigmoid(g), from the same bf16 inputs; the kernel's fast
+    exponential is part of the fp32 term."""
+    from harness import fused_ops
+
+    torch.manual_seed(5)
+    g = (torch.randn(3, 101, 704, device="cuda") * 3).to(torch.bfloat16).requires_grad_(True)
+    u = torch.randn(3, 101, 704, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    dy = torch.randn_like(g)
+    fused_ops.swiglu(g, u).backward(dy)
+    g64, u64, dy64 = _f64(g), _f64(u), _f64(dy)
+    sg = torch.sigmoid(g64)
+    dg = dy64 * u64 * sg * (1 + g64 * (1 - sg))
+    du = dy64 * g64 * sg
+    mag_g = (dy64 * u64).abs() * (sg + (g64 * sg * (1 - sg)).abs()) * (1 + g64.abs())   # __expf's error grows with |g|
+    _assert_elementwise(g.grad, dg, mag_g, 16, "swiglu d_gate")
+    _assert_elementwise(u.grad, du, du.abs() * (1 + g64.abs()), 16, "swiglu d_up")

@@ -176,3 +176,61 @@ def test_step_flat_equals_per_parameter_steps():
         for p, rp in zip(params, ref_params):
             assert torch.equal(p, rp), step
     assert float(opt._step_dev.item()) == 3
+
+
+def _flat_views(flat, shapes):
+    params, off = [], 0
+    for a, b in shapes:
+        params.append(torch.nn.Parameter(flat[off:off + a * b].view(a, b)))
+        off += a * b
+    return params
+
+
+@pytest.mark.parametrize("paged", [False, True])
+def test_step_flat_state_dict_resumes_bitwise(paged, tmp_path):
+    """optimizer.pt written after `step_flat` steps (the benchmarked configuration) holds the flat moments as per-parameter
+    slices and the device-side step count: a fresh optimizer loaded from it continues bit-identically to the uninterrupted
+    run.  The parameters are laid out in the flat buffer in another order than the optimizer lists them."""
+    import qlora_b200 as q
+
+    torch.manual_seed(5)
+    shapes = [(64, 40), (40, 64), (16, 128)]
+    n = sum(a * b for a, b in shapes)
+    w = (torch.randn(n, device="cuda") * 0.05).to(torch.bfloat16)
+    grads = [(torch.randn(n, device="cuda") * 0.01).to(torch.bfloat16) for _ in range(4)]
+    scales = [1.0, 0.5, 0.25, 1.0]
+    hp = dict(lr=1e-3, weight_decay=0.01, capturable=True, is_paged=paged)
+
+    def run(flat_p, opt, steps):
+        flat_g = torch.empty_like(flat_p)
+        scale = torch.ones((), device="cuda")
+        for g, sc in steps:
+            flat_g.copy_(g)
+            scale.fill_(sc)
+            opt.step_flat(flat_p, flat_g, grad_scale=scale)
+
+    flat_a = w.clone()
+    pa = _flat_views(flat_a, shapes)
+    run(flat_a, q.optim.AdamW(pa[::-1], **hp), list(zip(grads, scales)))
+    flat_b = w.clone()
+    pb = _flat_views(flat_b, shapes)
+    ob = q.optim.AdamW(pb[::-1], **hp)
+    run(flat_b, ob, list(zip(grads, scales))[:2])
+    sd = ob.state_dict()
+    assert sorted(sd["state"]) == [0, 1, 2] and all(float(st["step"]) == 2 for st in sd["state"].values())
+    f = tmp_path / "optimizer.pt"
+    torch.save(sd, f)
+    flat_c = flat_b.clone()
+    del ob, sd
+    pc = _flat_views(flat_c, shapes)
+    oc = q.optim.AdamW(pc[::-1], **hp)
+    oc.load_state_dict(torch.load(f, weights_only=True))
+    run(flat_c, oc, list(zip(grads, scales))[2:])
+    assert torch.equal(flat_c, flat_a)
+    assert float(oc._step_dev.item()) == 4
+    if paged:
+        assert oc._paged[id(oc._flat_key)][0].ptr == oc._flat[0].data_ptr()
+    m_c, v_c = oc._flat
+    assert all(torch.equal(st["state1"], m_c[off:off + p.numel()]) for st, p, off in
+               zip(oc.state_dict()["state"].values(), oc.param_groups[0]["params"], oc._flat_offsets))
+    assert torch.isfinite(v_c).all()
