@@ -106,10 +106,13 @@ int qb200_nf4_linear_bwd_dx(const void* dY, const uint8_t* packed, const uint8_t
 
 /* ---- K5 + LoRA (SURVEY.md 8f-1): the caller's low-rank update folded into the same launch ----------------
  * Replaces peft lora.Linear4bit.forward's  `result = base(x); result += lora_B(lora_A(x)) * scaling`  (two extra GEMMs and
- * two elementwise passes over [M,N]) by one extra bf16 contraction step accumulated in the same register accumulators:
+ * two elementwise passes over [M,N]) by ceil(R/64) extra bf16 contraction steps accumulated in the same register accumulators
+ * (ranks [64j, 64j+64) in step j, after the NF4 steps):
  *   forward : Y  = X . W^T (+bias) + U . V^T      U[M,R] = scaling * (X . A^T) (bf16),  V[N,R] = lora_B.weight
  *   backward: dX = dY . W          + U . Vt       U[M,R] = scaling * (dY . B)  (bf16),  Vt[R,K] = lora_A.weight
- * R: LoRA rank, a multiple of 8 in [8, 64] (columns/rows beyond R are zero-filled by TMA). */
+ * R: LoRA rank, a multiple of 8 in [8, 256] (columns/rows beyond R are zero-filled by TMA); every entry point that takes R
+ * (these two, _ex, _group, _group_scaled, _group_typed, _group_ex, _group_reuse) returns QB200_EUNSUPPORTED before any
+ * launch for any other nonzero R. */
 int qb200_nf4_linear_fwd_lora(const void* X, const uint8_t* packed, const uint8_t* absmax_u8, const float* code256,
                               const float* absmax2, const float* offset, const float* absmax_f32, const void* bias,
                               const void* U, const void* V, int64_t R, void* Y, int64_t M, int64_t N, int64_t K,

@@ -48,7 +48,7 @@ struct Params {
   int T, F, C;
   int K;                     // row pitch of W[N,K] in elements
   int N;                     // rows of W
-  int lora_r;                // > 0: one extra 16-bit contraction step per problem  Out += U_p[T,r] . V_p^T
+  int lora_r;                // > 0: ceil(r / 64) extra 16-bit contraction steps per problem  Out += U_p[T,r] . V_p^T
   int out_f32;               // 1: the drain writes fp32 (Linear4bit called with fp32 activations: no separate cast pass)
   float* ws;                 // split-K: fp32 partial sums [ksplit, T, F] (null otherwise)
   int debug;                 // ablation flags for performance triage (QB200_DEBUG_FLAGS; 0 in production):

@@ -371,7 +371,7 @@ static int plan_strip(const Params& p, Strip& s) {
   const int n_fb = (p.F + kUnitF - 1) / kUnitF;
   s.n_fbg = p.group_sum ? n_fb : n_fb * p.nprob;
   if (int64_t(s.n_fbg) * s.t_pad > INT32_MAX) return set_error(QB200_EUNSUPPORTED, "nf4_linear: M x N too large for one launch");
-  s.nsteps = (p.group_sum ? p.nprob : 1) * ((p.C + kBlockC - 1) / kBlockC + (p.lora_r > 0 ? 1 : 0));
+  s.nsteps = (p.group_sum ? p.nprob : 1) * ((p.C + kBlockC - 1) / kBlockC + (p.lora_r + kBlockC - 1) / kBlockC);
   return 0;
 }
 
@@ -625,8 +625,8 @@ static int linear_group(int is_bwd, int dtype, int state_dtype, int out_dtype, i
   if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
   int rc = gemm::validate_shape(M, N, K);
   if (rc) return rc;
-  if (R != 0 && (R < 0 || R > 64 || R % 8 != 0))
-    return set_error(QB200_EUNSUPPORTED, "nf4_linear_lora: rank must be a multiple of 8 in [8, 64]");
+  if (R != 0 && (R < 0 || R > kMaxLoraRank || R % 8 != 0))
+    return set_error(QB200_EUNSUPPORTED, "nf4_linear_lora: rank must be a multiple of 8 in [8, 256]");
   const bool nested = probs[0].absmax_u8 != nullptr;
   for (int i = 0; i < nprob; ++i) {
     rc = gemm::validate_problem(probs[i], is_bwd, R, N, K, !(is_bwd && i > 0));

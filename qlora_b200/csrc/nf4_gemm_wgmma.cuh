@@ -27,9 +27,9 @@
 //
 // Barrier protocol (shared memory of the CTA):
 //   full_in[s]  arrive.expect_tx + TMA complete_tx (issued by the dequant group of the step) -> consumers
-//   full_a[s]   4 dequant-warp arrivals (or the group's LoRA V tile, lora_bar)           -> consumers
+//   full_a[s]   4 dequant-warp arrivals (LoRA step: warp 0's after its lora_bar wait)   -> consumers
 //   empty[s]    8 consumer-warp arrivals once the step's wgmma group has completed      -> dequantizers
-//   lora_bar[g] TMA of a LoRA V tile into an A slot, one barrier per dequant group      -> that group
+//   lora_bar[g] TMA of a LoRA V tile into an A slot, one barrier per dequant group      -> the group's first thread
 // The consumers keep one wgmma group in flight: step g's slot is released after wgmma.wait_group 1 in step g + 1.
 //
 // Programmatic dependent launch: the kernel is launched with programmatic stream serialization, signals
@@ -74,13 +74,13 @@ struct Work {
   int kb0;     // first NF4 contraction step
   int nkb;     // NF4 contraction steps per segment
   int nseg;    // contraction segments (contraction-sum groups: one per problem)
-  int lora;    // 1: a 16-bit LoRA step follows the NF4 steps of every segment
+  int lora;    // 16-bit LoRA steps (ceil(r / 64), ranks [64 j, 64 j + 64) each) after the NF4 steps of every segment
   int split;   // split-K index (0 when the unit covers the whole contraction)
 };
 
 // Decode the unit at cursor `a` of a CTA whose range ends at `end`.
 __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const Sched& sched, const Params& p, int num_kb,
-                                            int has_lora) {
+                                            int n_lora) {
   Work w;
   int fb;
   if (sched.ksplit > 1) {
@@ -89,7 +89,7 @@ __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const 
     const int per = (num_kb + sched.ksplit - 1) / sched.ksplit;
     w.kb0 = w.split * per;
     w.nkb = (num_kb - w.kb0) < per ? (num_kb - w.kb0) : per;
-    w.lora = (has_lora && w.split == 0) ? 1 : 0;
+    w.lora = w.split == 0 ? n_lora : 0;
     fb = tile / sched.n_tt;
     w.t0 = (tile - fb * sched.n_tt) * kUnitT;
     const int rem = p.T - w.t0;                          // few-token calls issue narrow MMAs and store only what exists
@@ -118,7 +118,7 @@ __device__ __forceinline__ Work decode_work(int a, int end, int num_ctas, const 
     w.split = 0;
     w.kb0 = 0;
     w.nkb = num_kb;
-    w.lora = has_lora;
+    w.lora = n_lora;
   }
   w.f0 = fb * kUnitF;
   return w;
@@ -244,7 +244,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
   const int lane = threadIdx.x & 31;
   const int num_ctas = gridDim.x;
   const int num_kb = (p.C + kBlockC - 1) / kBlockC;
-  const int has_lora = p.lora_r > 0 ? 1 : 0;
+  const int n_lora = (p.lora_r + kBlockC - 1) / kBlockC;   // LoRA steps per segment
   // this CTA's cursor range: unit indices (split-K) or token-rows of the output strip (range schedule)
   const int cur0 = sched.ksplit > 1 ? int(blockIdx.x) : sched.start[blockIdx.x];
   const int cur_end = sched.ksplit > 1 ? sched.n_work : sched.start[blockIdx.x + 1];
@@ -252,7 +252,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.nprob; ++i) {
       ptx::tma_prefetch_desc(&maps.in[i]);
-      if (has_lora) {
+      if (n_lora) {
         ptx::tma_prefetch_desc(&maps.u[i]);
         ptx::tma_prefetch_desc(&maps.v[i]);
       }
@@ -314,8 +314,8 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
       return int64_t(n) * kblocks_per_row + (kcol >> 6);
     };
     // Iterator over this group's steps (global step g = group, group + kNumGroups, ...) across the CTA's units: (seg, i) = segment
-    // and step-in-segment inside the current unit `u` (i < u.nkb: NF4 step kb = u.kb0 + i, i == u.nkb: the segment's LoRA
-    // step).  Units are decoded only when the cursor moves to the next one.
+    // and step-in-segment inside the current unit `u` (i < u.nkb: NF4 step kb = u.kb0 + i, i >= u.nkb: the segment's LoRA
+    // step i - u.nkb).  Units are decoded only when the cursor moves to the next one.
     int cur = cur0, seg = 0, i = 0;
     uint32_t lora_cnt = 0;                   // LoRA steps this group has handled (phase of its lora_bar)
     Work u{};
@@ -332,14 +332,14 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
         if (seg < u.nseg) return;
         cur = u.next;                        // past the end of the unit: i steps into the next one
         if (cur >= cur_end) return;
-        u = decode_work(cur, cur_end, num_ctas, sched, p, num_kb, has_lora);
+        u = decode_work(cur, cur_end, num_ctas, sched, p, num_kb, n_lora);
         per = u.nkb + u.lora;
         seg = 0;
         fresh = true;
       }
     };
     if (cur < cur_end) {
-      u = decode_work(cur, cur_end, num_ctas, sched, p, num_kb, has_lora);
+      u = decode_work(cur, cur_end, num_ctas, sched, p, num_kb, n_lora);
       per = u.nkb + u.lora;
       advance(group);
     }
@@ -406,35 +406,40 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(full_a(sa));
       } else {
-        // LoRA step: the A-operand tile is plain T16 (V rows of this unit's 128 features x r), TMA'd straight into the A
-        // slot in the same canonical layout the dequantizers produce (K-major fwd / MN-major dX).
+        // LoRA step j = i - u.nkb: the A-operand tile is plain T16 (V of this unit's 128 features x ranks [64 j, 64 j + 64)),
+        // TMA'd straight into the A slot in the same canonical layout the dequantizers produce (K-major fwd / MN-major dX).
+        // Only the issuing thread waits for the tile, so lora_bar has one waiter, which re-arms it only after its own wait:
+        // its phase cannot run ahead of any waiter, however many LoRA steps a group takes in a row.  The other warps write
+        // nothing in this step and arrive at once; full_a completes with warp 0's arrival, after the tile has landed.
         const int lora_pi = p.group_sum ? seg : u.prob;
+        const int lc = (i - u.nkb) * kBlockC;
         ptx::mbar_wait(empty(sa), empty_ph);
         if (t == 0) {
           ptx::grid_dep_wait();   // the adapters are written by the optimizer step
           ptx::mbar_arrive_expect_tx(lora_bar(group), kATileBytes);
           if (!kTrans) {
-            ptx::tma_load_2d(a_tile(sa), &maps.v[lora_pi], lora_bar(group), 0, u.f0);                   // V[F, r]: box {64, 128}
+            ptx::tma_load_2d(a_tile(sa), &maps.v[lora_pi], lora_bar(group), lc, u.f0);                  // V[F, r]: box {64, 128}
           } else {
-            ptx::tma_load_2d(a_tile(sa), &maps.v[lora_pi], lora_bar(group), u.f0, 0);                   // Vt[r, F]: 2 x box {64, 64}
-            ptx::tma_load_2d(a_tile(sa) + 8192u, &maps.v[lora_pi], lora_bar(group), u.f0 + 64, 0);
+            ptx::tma_load_2d(a_tile(sa), &maps.v[lora_pi], lora_bar(group), u.f0, lc);                  // Vt[r, F]: 2 x box {64, 64}
+            ptx::tma_load_2d(a_tile(sa) + 8192u, &maps.v[lora_pi], lora_bar(group), u.f0 + 64, lc);
           }
+          ptx::mbar_wait(lora_bar(group), lora_cnt & 1u);
+          ++lora_cnt;
         }
-        ptx::mbar_wait(lora_bar(group), lora_cnt & 1u);
-        ++lora_cnt;
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(full_a(sa));
       }
       if (t == 0) {
-        // this step's activation block (LoRA step: U[T, r], columns >= r zero-filled); the box is always 128 rows: rows past
-        // T are zero-filled, rows past the unit are loaded but not multiplied.  Issued after the A tile so that the first
-        // steps' dequantization overlaps the previous kernel; the slot is free (empty[sa] was waited for above).
+        // this step's activation block (LoRA step j: columns [64 j, 64 j + 64) of U[T, r], columns >= r zero-filled); the box
+        // is always 128 rows: rows past T are zero-filled, rows past the unit are loaded but not multiplied.  Issued after
+        // the A tile so that the first steps' dequantization overlaps the previous kernel; the slot is free (empty[sa] was
+        // waited for above).
         ptx::grid_dep_wait();   // activations / U come from earlier kernels
         const int pi = p.group_sum ? seg : u.prob;
         const bool lora_step = i >= u.nkb;
         ptx::mbar_arrive_expect_tx(full_in(sa), kInSlotBytes);
-        ptx::tma_load_2d(in_tile(sa), lora_step ? &maps.u[pi] : &maps.in[pi], full_in(sa), lora_step ? 0 : (u.kb0 + i) * kBlockC,
-                         u.t0);
+        ptx::tma_load_2d(in_tile(sa), lora_step ? &maps.u[pi] : &maps.in[pi], full_in(sa),
+                         (lora_step ? i - u.nkb : u.kb0 + i) * kBlockC, u.t0);
       }
       advance(kNumGroups);
       prefetch_step();      // loads of this group's next step fly while the other groups run
@@ -447,7 +452,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
 #pragma unroll
     for (int i = 0; i < ptx::kWgmmaMaxAcc; ++i) acc[i] = 0.0f;
     for (int a = cur0; a < cur_end;) {
-      const Work w = decode_work(a, cur_end, num_ctas, sched, p, num_kb, has_lora);
+      const Work w = decode_work(a, cur_end, num_ctas, sched, p, num_kb, n_lora);
       a = w.next;
       switch (w.nt >> 4) {
         case 1: consume_unit<T16, 16, kTrans, kOutF16>(w, p, sched, wg, warp, lane, smem_base, aux, g, acc); break;
@@ -473,7 +478,7 @@ nf4_gemm_wgmma_kernel(const __grid_constant__ Maps maps, const __grid_constant__
 // Units are 128 features x up to 256 tokens (wgmma m64nNk16, N <= 256, one M=64 half per consumer warpgroup), with the same
 // LoRA step, grouped forms and output arithmetic as the fused kernel above; the A tile of a step is the same 16 KB K-major (forward)
 // or MN-major (dX) tile the dequantizers build, loaded from the scratch instead.  Each output element sums the same products
-// in the same order (NF4 steps in order, then the LoRA step) as the fused kernel.
+// in the same order (NF4 steps in order, then the LoRA steps of ranks 0-63, 64-127, ...) as the fused kernel.
 //
 // Schedule (sc::Sched, host: launch_scratch_gemm).  The units are the 256-token tiles of the n_fb x T strip, numbered
 // feature-block-major with the token tile fastest.  CTA c runs units c, c + P, c + 2P, ... (P = gridDim.x) for the full
@@ -537,7 +542,7 @@ __device__ __forceinline__ int unit_row(int u, const Sched& sched) {
 }
 
 // Decode the unit at cursor `a` of a CTA whose tail range ends at `end`.
-__device__ __forceinline__ Work decode_work(int a, int end, const Sched& sched, const Params& p, int num_kb, int has_lora) {
+__device__ __forceinline__ Work decode_work(int a, int end, const Sched& sched, const Params& p, int num_kb, int n_lora) {
   Work w;
   const int fbg = a / sched.t_pad;
   w.t0 = a - fbg * sched.t_pad;
@@ -563,7 +568,7 @@ __device__ __forceinline__ Work decode_work(int a, int end, const Sched& sched, 
   w.split = 0;
   w.kb0 = 0;
   w.nkb = num_kb;
-  w.lora = has_lora;
+  w.lora = n_lora;
   return w;
 }
 
@@ -674,7 +679,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_kb = (p.C + kBlockC - 1) / kBlockC;
-  const int has_lora = p.lora_r > 0 ? 1 : 0;
+  const int n_lora = (p.lora_r + kBlockC - 1) / kBlockC;   // LoRA steps per segment
   const int cur0 = sched.n_rr > 0 ? unit_row(int(blockIdx.x), sched) : sched.start[blockIdx.x];
   const int cur_end = sched.start[blockIdx.x + 1];
 
@@ -683,7 +688,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
       ptx::tma_prefetch_desc(&maps.in[i]);
       ptx::tma_prefetch_desc(&maps.w[i]);
       if (!p.out_f32) ptx::tma_prefetch_desc(&maps.out[i]);
-      if (has_lora) {
+      if (n_lora) {
         ptx::tma_prefetch_desc(&maps.u[i]);
         ptx::tma_prefetch_desc(&maps.v[i]);
       }
@@ -704,7 +709,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
       ptx::grid_dep_wait();   // the scratch, the activations and the adapters are outputs of earlier kernels
       uint32_t g = 0;
       for (int a = cur0; a < cur_end;) {
-        const Work w = decode_work(a, cur_end, sched, p, num_kb, has_lora);
+        const Work w = decode_work(a, cur_end, sched, p, num_kb, n_lora);
         a = w.next;
         for (int seg = 0; seg < w.nseg; ++seg) {
           const int pi = p.group_sum ? seg : w.prob;
@@ -712,10 +717,11 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
             const int s = int(g % kStages);
             ptx::mbar_wait(empty(s), ((g / kStages) & 1) ^ 1);
             ptx::mbar_arrive_expect_tx(full(s), kATileBytes + kInSlotBytes);
-            // A: the step's 128 features x 64 contraction of W (or the unit's LoRA V tile), in the consumers' layout
+            // A: the step's 128 features x 64 contraction of W (or, LoRA step i - nkb, the unit's V tile of those 64 ranks), in
+            // the consumers' layout
             const bool lora = i >= w.nkb;
             const CUtensorMap* am = lora ? &maps.v[pi] : &maps.w[pi];
-            const int c = lora ? 0 : (w.kb0 + i) * kBlockC;
+            const int c = (lora ? i - w.nkb : w.kb0 + i) * kBlockC;
             if (!kTrans) {
               ptx::tma_load_2d(a_tile(s), am, full(s), c, w.f0);
             } else {
@@ -738,7 +744,7 @@ nf4_scratch_gemm_kernel(const __grid_constant__ Maps maps, const __grid_constant
 #pragma unroll
     for (int i = 0; i < ptx::kWgmmaWideAcc; ++i) acc[i] = 0.0f;
     for (int a = cur0; a < cur_end;) {
-      const Work w = decode_work(a, cur_end, sched, p, num_kb, has_lora);
+      const Work w = decode_work(a, cur_end, sched, p, num_kb, n_lora);
       a = w.next;
       // N: the unit's tokens rounded up to 16 up to 128, to 32 above
       if (w.nt <= 128) {

@@ -71,31 +71,35 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a
 #undef QB200_MMA_16816
 
 // LoRA term of one output value: sum_j U[m, j] * V[row, j] over the rank (T16 operands, fp32 sum) — the extra contraction
-// step the wgmma kernel runs on the tensor core, here 8..64 multiply-adds in the epilogue.  U = scaling * x . A^T [M, r] comes
-// from the caller (one small GEMM), V = lora_B.weight [N, r]; rows are 16-byte aligned (r % 8 == 0).
+// steps the wgmma kernel runs on the tensor core, here 8..256 multiply-adds in the epilogue.  U = scaling * x . A^T [M, r]
+// comes from the caller (one small GEMM), V = lora_B.weight [N, r]; rows are 16-byte aligned (r % 8 == 0).
 template <typename T16>
 __device__ __forceinline__ float lora_dot(const T16* __restrict__ u, const T16* __restrict__ v, int r) {
   using T2 = typename Vec2<T16>::type;
-  // all (at most 8 + 8) 16-byte loads are issued before the first multiply: one memory round trip, not r / 8 of them
-  uint4 a[8], b[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (8 * i < r) {
-      a[i] = *reinterpret_cast<const uint4*>(u + 8 * i);          // produced by the previous kernel: plain load
-      b[i] = __ldg(reinterpret_cast<const uint4*>(v + 8 * i));
-    }
-  }
   float acc = 0.0f;
+  // chunks of 64 ranks, summed in rank order into one accumulator: r <= 64 is one chunk, the sum it always was
+  for (int c0 = 0; c0 < r; c0 += 64) {
+    // all (at most 8 + 8) 16-byte loads of the chunk are issued before its first multiply: one memory round trip per
+    // chunk, not r / 8 of them
+    uint4 a[8], b[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (8 * i < r) {
-      const T2* a2 = reinterpret_cast<const T2*>(&a[i]);
-      const T2* b2 = reinterpret_cast<const T2*>(&b[i]);
+    for (int i = 0; i < 8; ++i) {
+      if (c0 + 8 * i < r) {
+        a[i] = *reinterpret_cast<const uint4*>(u + c0 + 8 * i);     // produced by the previous kernel: plain load
+        b[i] = __ldg(reinterpret_cast<const uint4*>(v + c0 + 8 * i));
+      }
+    }
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 fa = widen2(a2[e]), fb = widen2(b2[e]);
-        acc = fmaf(fa.x, fb.x, acc);
-        acc = fmaf(fa.y, fb.y, acc);
+    for (int i = 0; i < 8; ++i) {
+      if (c0 + 8 * i < r) {
+        const T2* a2 = reinterpret_cast<const T2*>(&a[i]);
+        const T2* b2 = reinterpret_cast<const T2*>(&b[i]);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 fa = widen2(a2[e]), fb = widen2(b2[e]);
+          acc = fmaf(fa.x, fb.x, acc);
+          acc = fmaf(fa.y, fb.y, acc);
+        }
       }
     }
   }
@@ -434,21 +438,37 @@ nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ pa
     s_red[warp * kRows + 2 * t + 1] = acc[0][1] + acc[1][3];
   }
   if (lora_r > 0) {
-    // 16 lanes per weight row, 4 rank entries each (r <= 64), summed by xor-shuffles: the loads overlap the barrier
+    // 16 lanes per weight row, 4 rank entries of each 64-rank chunk each (r <= 256: up to 4 chunks), every chunk summed by
+    // xor-shuffles and the chunk sums added in rank order (r <= 64: one chunk, the sum it always was).  All loads are issued
+    // before the first multiply; they overlap the barrier.
+    constexpr int kChunks = kMaxLoraRank / 64;
     const int row = threadIdx.x >> 4, c = (threadIdx.x & 15) << 2;
-    float part = 0.0f;
-    if (row < kRows && c < lora_r) {
-      const uint2 a = *reinterpret_cast<const uint2*>(lora_u + c);
-      const uint2 b = __ldg(reinterpret_cast<const uint2*>(lora_v + int64_t(blockIdx.x * kRows + row) * lora_r + c));
-      const float2 a0 = widen2(*reinterpret_cast<const T2*>(&a.x));
-      const float2 a1 = widen2(*reinterpret_cast<const T2*>(&a.y));
-      const float2 b0 = widen2(*reinterpret_cast<const T2*>(&b.x));
-      const float2 b1 = widen2(*reinterpret_cast<const T2*>(&b.y));
-      part = fmaf(a0.x, b0.x, fmaf(a0.y, b0.y, fmaf(a1.x, b1.x, a1.y * b1.y)));
-    }
+    const T16* vrow = lora_v + int64_t(blockIdx.x * kRows + row) * lora_r;
+    uint2 a[kChunks], b[kChunks];
 #pragma unroll
-    for (int o = 8; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    if (row < kRows && (threadIdx.x & 15) == 0) s_red[kWarps * kRows + row] = part;
+    for (int k = 0; k < kChunks; ++k) {
+      if (row < kRows && 64 * k + c < lora_r) {
+        a[k] = *reinterpret_cast<const uint2*>(lora_u + 64 * k + c);
+        b[k] = __ldg(reinterpret_cast<const uint2*>(vrow + 64 * k + c));
+      }
+    }
+    float sum = 0.0f;
+#pragma unroll
+    for (int k = 0; k < kChunks; ++k) {
+      if (64 * k >= lora_r) break;
+      float part = 0.0f;
+      if (row < kRows && 64 * k + c < lora_r) {
+        const float2 a0 = widen2(*reinterpret_cast<const T2*>(&a[k].x));
+        const float2 a1 = widen2(*reinterpret_cast<const T2*>(&a[k].y));
+        const float2 b0 = widen2(*reinterpret_cast<const T2*>(&b[k].x));
+        const float2 b1 = widen2(*reinterpret_cast<const T2*>(&b[k].y));
+        part = fmaf(a0.x, b0.x, fmaf(a0.y, b0.y, fmaf(a1.x, b1.x, a1.y * b1.y)));
+      }
+#pragma unroll
+      for (int o = 8; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+      sum = k == 0 ? part : sum + part;
+    }
+    if (row < kRows && (threadIdx.x & 15) == 0) s_red[kWarps * kRows + row] = sum;
   }
   __syncthreads();
   if (threadIdx.x < kRows) {
@@ -502,7 +522,7 @@ static int launch_chunks(qb200_nf4_problem q, const float* row_scale, int M, int
 // Internal: forward skinny GEMM, 16 tokens per launch, with the skinny kernels of `kernels`; optional LoRA term
 // y += U[M,R] . V[N,R]^T  (R = 0: none); optional row_scale[N] (null: none) multiplies row n of W; in / out / U may be column
 // slices of wider row-major buffers (row pitches ld_in / ld_out / ld_u in elements, 0 = dense); caller has validated
-// pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0, R <= 64, 16-byte aligned in / U rows and V).
+// pointers/shapes (K % 64 == 0, N % 8 == 0, R % 8 == 0, R <= kMaxLoraRank = 256, 16-byte aligned in / U rows and V).
 int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int M, int N, int K, int R, Nf4Kernels kernels,
                       cudaStream_t stream) {
   if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");

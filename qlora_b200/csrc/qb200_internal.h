@@ -81,6 +81,10 @@ auto with_nf4_types(Nf4Kernels k, Fn&& fn) {
   return fn(Nf4Types<BF, false, false>{});
 }
 
+// LoRA ranks of the NF4 linear entry points: multiples of 8 up to this.  The wgmma kernels contract them in one 64-wide step
+// per 64 ranks, the skinny kernels in 64-rank chunks of their epilogue.
+constexpr int kMaxLoraRank = 256;
+
 // Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16 and a 16-bit output: problem q with its
 // optional LoRA term U[M,R] . V[N,R]^T (R = 0: none) and an optional per-row weight scale row_scale[N] (null: none), run by
 // the skinny kernels of `kernels`.

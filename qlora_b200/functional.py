@@ -690,8 +690,13 @@ def nf4_linear_bwd_dx(dy2d: Tensor, packed: Tensor, quant_state: QuantState, out
     return _linear_ex(True, dy2d, packed, quant_state, out_dtype=out_dtype)
 
 
+LORA_MAX_RANK = 256
+
+
 def lora_fused_supported(quant_state: QuantState, compute_dtype: torch.dtype, r: int) -> bool:
-    return fused_supported(quant_state, compute_dtype) and 8 <= r <= 64 and r % 8 == 0
+    """Whether the fused kernels take a LoRA term of rank r over this state: r a multiple of 8 (16-byte TMA rows) up to
+    256, contracted in one 64-wide step per 64 ranks (one 64-rank chunk of the epilogue on the skinny kernels)."""
+    return fused_supported(quant_state, compute_dtype) and 8 <= r <= LORA_MAX_RANK and r % 8 == 0
 
 
 def nf4_linear_fwd_lora(x2d: Tensor, packed: Tensor, quant_state: QuantState, u: Tensor, v: Tensor,

@@ -12,7 +12,8 @@ update is ONE extra 16-bit contraction step of the fused kernel, accumulated in 
     backward: dX = dY . W  + G . A           G = scaling * (dY . B)          [M, r]
               dA = G^T . drop(X)   dB = dY^T . U                             (the trainable adapters' grads)
 
-Only the skinny [M, r] projections stay separate (cuBLAS).  The sum is rounded to the compute dtype once (the unfused
+Ranks of 8..256 (multiples of 8) are one 64-wide contraction step per 64 ranks.  Only the skinny [M, r] projections stay
+separate (cuBLAS).  The sum is rounded to the compute dtype once (the unfused
 sequence rounds the base output and the update separately), so results agree with peft's to within one ulp of it.
 The compute dtype is bf16 (over a bf16 or fp16 quant state), or fp16 for a base with `compute_dtype=torch.float16` (over an
 fp16 or fp32 quant state); the adapters are of the compute dtype.  fp16 activations under bf16 compute, and fp32 states
@@ -227,7 +228,7 @@ def lora_linear4bit(x: torch.Tensor, base, lora_a: torch.Tensor, lora_b: torch.T
 
     `x_lora` is the LoRA branch's input when it differs from `x` (peft applies dropout to it); None = `x`.
     Falls back to the two-step form (still on the GPU kernels) when the fused kernel does not cover the case
-    (fp32 compute dtype, rank not a multiple of 8 or > 64, bias present, unsupported shape or quant-state dtype)."""
+    (fp32 compute dtype, rank not a multiple of 8 or > 256, bias present, unsupported shape or quant-state dtype)."""
     x_loras = None if x_lora is None else [x_lora]
     if _group_fusable(x, [base], [lora_a], [lora_b], x_loras):
         return _apply(LoraMatMul4Bit, x, [base], scaling, x_loras, [lora_a], [lora_b])[0]
