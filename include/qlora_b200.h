@@ -240,6 +240,24 @@ int qb200_adamw32bit_step(void* p, int dtype, const void* g, float* m, float* v,
 int qb200_adamw32bit_step_dev(void* p, int dtype, const void* g, float* m, float* v, int64_t n, float lr, float beta1,
                               float beta2, float eps, float weight_decay, const float* step_dev, const float* gnorm_scale_dev,
                               void* stream);
+/* ---- 32-bit Lion, RMSprop and AdEMAMix (optim='lion_32bit', 'rmsprop_bnb', 'ademamix' and their paged forms) -----------
+ * Replace clion32bit_grad_*, crmsprop32bit_grad_* (kOptimizer32bit1State<T, LION | RMSPROP>) and cademamix32bit_grad_*
+ * (kOptimizer32bit2State<T, ADEMAMIX>).  One fused elementwise pass each: p, g of `dtype`; state fp32; every operation a
+ * correctly rounded fp32 one.  `gnorm_scale_dev` is an optional DEVICE float multiplying the gradient.  They allocate nothing
+ * and read no host state per step, so one captured launch can be replayed every step.
+ *   Lion:     c = b1*m + (1-b1)*g; if (wd > 0) p *= 1 - lr*wd; p -= lr*sign(c); m = b2*m + (1-b2)*g.  `step_dev` is unused.
+ *   RMSprop:  if (wd > 0) g += wd*p; v = alpha*v + (1-alpha)*g*g; p -= lr*(g / (sqrt(v) + eps)).  `step_dev` is unused.
+ *   AdEMAMix: `step_dev` is a DEVICE float holding the step count t (from 1); m1, m2 the fast and slow EMAs, nu the second
+ *             moment.  t_alpha, t_beta3 > 0 set the warm-up schedules of alpha and beta3, 0 means none; a negative or NaN
+ *             value returns QB200_EINVAL.
+ * Null pointers, n < 0 and an unknown dtype return QB200_EINVAL before any launch. */
+int qb200_lion32bit_step_dev(void* p, int dtype, const void* g, float* m, int64_t n, float lr, float beta1, float beta2,
+                             float weight_decay, const float* step_dev, const float* gnorm_scale_dev, void* stream);
+int qb200_rmsprop32bit_step_dev(void* p, int dtype, const void* g, float* v, int64_t n, float lr, float alpha, float eps,
+                                float weight_decay, const float* step_dev, const float* gnorm_scale_dev, void* stream);
+int qb200_ademamix32bit_step_dev(void* p, int dtype, const void* g, float* m1, float* m2, float* nu, int64_t n, float lr, float beta1,
+                                 float beta2, float beta3, float alpha, float t_alpha, float t_beta3, float eps, float weight_decay,
+                                 const float* step_dev, const float* gnorm_scale_dev, void* stream);
 int qb200_managed_alloc(int64_t bytes, void** out);
 int qb200_managed_free(void* ptr);
 int qb200_prefetch(const void* ptr, int64_t bytes, int device, void* stream);

@@ -41,6 +41,9 @@ _SIGS = {
                                ct.c_float, _vp], _i32),
     "qb200_adamw32bit_step_dev": ([_vp, _i32, _vp, _vp, _vp, _i64, ct.c_float, ct.c_float, ct.c_float, ct.c_float, ct.c_float, _vp, _vp,
                                    _vp], _i32),
+    "qb200_lion32bit_step_dev": ([_vp, _i32, _vp, _vp, _i64] + [ct.c_float] * 4 + [_vp, _vp, _vp], _i32),
+    "qb200_rmsprop32bit_step_dev": ([_vp, _i32, _vp, _vp, _i64] + [ct.c_float] * 4 + [_vp, _vp, _vp], _i32),
+    "qb200_ademamix32bit_step_dev": ([_vp, _i32, _vp, _vp, _vp, _vp, _i64] + [ct.c_float] * 9 + [_vp, _vp, _vp], _i32),
     "qb200_managed_alloc": ([_i64, ct.POINTER(ct.c_void_p)], _i32),
     "qb200_managed_free": ([_vp], _i32),
     "qb200_prefetch": ([_vp, _i64, _i32, _vp], _i32),
