@@ -124,8 +124,9 @@ int qb200_nf4_linear_bwd_dx_lora(const void* dY, const uint8_t* packed, const ui
 /* ---- general form: optional LoRA operands (R = 0: none) and optional split-K workspace -----------------------
  * For very small token counts the contraction is split over several clusters; the fp32 partial sums need a caller-lent
  * DEVICE workspace of qb200_nf4_linear_workspace_size() bytes (0 = not needed).  Without a workspace the un-split
- * schedule is used.  is_bwd: 0 forward (in = X, out = Y, V = lora_B.weight [N,R]), 1 backward-dX (in = dY, out = dX,
- * V = lora_A.weight [R,K]; bias must be NULL). */
+ * schedule is used, as it is for an output whose base is not 8-byte (16-bit output) or 16-byte (fp32 output) aligned or
+ * whose row pitch is not a multiple of 4 elements.  is_bwd: 0 forward (in = X, out = Y, V = lora_B.weight [N,R]),
+ * 1 backward-dX (in = dY, out = dX, V = lora_A.weight [R,K]; bias must be NULL). */
 int64_t qb200_nf4_linear_workspace_size(int64_t M, int64_t N, int64_t K, int is_bwd);
 /* Training token counts: at M >= a threshold (default 1536, env QB200_SCRATCH_MIN_M) a call in bf16 compute over a bf16 or fp32
  * state, with a bf16 or fp32 output and no row scale, writes each of its nprob weights once as bf16 [N,K] into the caller-lent

@@ -443,10 +443,14 @@ static int launch_gemm(const GroupArgs& g, cudaStream_t stream) {
   const int ctas = num_ctas();
   Sched sched{};
   int n_ctas;
-  // split-K only for single problems whose caller lent a large enough fp32 workspace [ksplit, T, F]
+  // split-K only for single problems whose caller lent a large enough fp32 workspace [ksplit, T, F], and whose output the
+  // reduce's 4-feature vector stores can reach: F and the row pitch multiples of 4, the base 8-byte (16-bit output) or
+  // 16-byte (fp32 output) aligned
   int ksplit = g.nprob == 1 ? plan_ksplit(T, F, C) : 1;
+  const uintptr_t out_align = p.out_f32 ? 16 : 8;
   if (ksplit > 1 && (g.workspace == nullptr || g.workspace_bytes < int64_t(ksplit) * T * F * 4 ||
-                     reinterpret_cast<uintptr_t>(g.workspace) % 16 != 0 || F % 4 != 0 || p.pr[0].ld_out % 4 != 0))
+                     reinterpret_cast<uintptr_t>(g.workspace) % 16 != 0 || F % 4 != 0 || p.pr[0].ld_out % 4 != 0 ||
+                     reinterpret_cast<uintptr_t>(p.pr[0].out) % out_align != 0))
     ksplit = 1;
   if (ksplit > 1) {
     sched.ksplit = ksplit;
