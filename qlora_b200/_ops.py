@@ -1,0 +1,412 @@
+"""The library's launches as torch custom ops (namespace `qlora_b200`), so that `torch.compile` traces through them.
+
+Every device call of `functional` goes through one of these ops, in eager mode as under compile: the ctypes calls into
+libqlora_b200.so live in the ops' implementations only.  Each op has a fake kernel that states its outputs' shapes, dtypes
+and strides and runs the same argument checks as the launch, so a rejected call raises at trace time as it does eagerly.
+
+A `QuantState` is not a valid op argument: the ops take its tensors (absmax, and for a nested state the second-level code,
+absmax and offset) plus plain ints.  Outputs that a caller lends (`outs`, `out`, `absmax`) are declared in `mutates_args`.
+The choice between the skinny, split-K, fused and scratch kernels (inside the C library) and between the library's LoRA
+projection and cuBLAS (`lora_project`) is made inside the ops at every call, never by a Python branch on the token count,
+so a graph traced with a symbolic token count serves every count (tests/test_gpu_compile.py checks two lengths, one
+compilation).
+"""
+from __future__ import annotations
+
+import ctypes as ct
+from typing import Optional
+
+import torch
+from torch import Tensor
+
+from . import _lib
+from . import functional as F
+from ._lib import DTYPE_CODE, check, ptr, stream_ptr
+
+BLOCKSIZES = (4096, 2048, 1024, 512, 256, 128, 64)
+
+
+def _device(*tensors: Optional[Tensor]) -> torch.device:
+    """The one CUDA device of the tensors (None entries skipped)."""
+    dev = None
+    for t in tensors:
+        if t is None:
+            continue
+        if not t.is_cuda:
+            raise RuntimeError(
+                "qlora_b200 ops run on CUDA tensors only (H100-native kernels, no CPU fallback); "
+                f"got a tensor on {t.device}"
+            )
+        if dev is None:
+            dev = t.device
+        elif t.device != dev:
+            raise RuntimeError(f"all tensors must be on the same GPU, found {dev} and {t.device}")
+    if dev is None:
+        raise RuntimeError("no tensors given")
+    return dev
+
+
+def _check_blocksize(blocksize: int) -> None:
+    if blocksize not in BLOCKSIZES:
+        raise ValueError(f"blocksize {blocksize} not in {BLOCKSIZES}")
+
+
+def _check_state(absmax: Tensor, code2: Optional[Tensor], absmax2: Optional[Tensor], offset: Optional[Tensor]) -> None:
+    """The state tensors as the kernels read them: uint8 codes with fp32 code / absmax2 / offset (nested), or fp32 absmax."""
+    nested = code2 is not None
+    assert (absmax2 is not None) == nested and (offset is not None) == nested, "nested state: code2, absmax2 and offset"
+    if nested:
+        assert absmax.dtype == torch.uint8 and code2.dtype == absmax2.dtype == offset.dtype == torch.float32, \
+            "nested state: uint8 absmax, fp32 code2 / absmax2 / offset"
+        assert code2.is_contiguous() and absmax2.is_contiguous(), "nested state tensors must be contiguous"
+    else:
+        assert absmax.dtype == torch.float32, "plain state: fp32 absmax"
+    assert absmax.is_contiguous(), "absmax must be contiguous"
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the grouped NF4 linear: forward and dX of 1..3 Linear4bit of one shape in one launch
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _check_group(is_bwd, inputs, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, us, vs, outs,
+                 out_dtype, row_scales, w_scratch):
+    """Argument rules of `qb200_nf4_linear_group_reuse` / `_typed`, checked before any launch (and by the fake kernel).
+    Returns (device, m, r, c_in, f_out, compute dtype, double-rounded weights, fused-kernel-only variant)."""
+    n = len(packeds)
+    assert 1 <= n <= 3 and len(inputs) == n and len(absmax) == n and len(code2) == n and len(absmax2) == n \
+        and len(offset) == n, "1..3 problems, with one input and one state each"
+    dev = _device(*inputs, *packeds, *absmax, *code2, *absmax2, *offset)
+    for i in range(n):
+        _check_state(absmax[i], code2[i], absmax2[i], offset[i])
+    assert len({c is None for c in code2}) == 1, "grouped problems must share their quantization form"
+    c_in, f_out = (n_out, k_in) if is_bwd else (k_in, n_out)
+    m = inputs[0].shape[0]
+    cdt = inputs[0].dtype
+    assert cdt in (torch.bfloat16, torch.float16), f"inputs: bf16 or fp16, got {cdt}"
+    for t in inputs:
+        assert t.dim() == 2 and t.shape == (m, c_in) and t.dtype == cdt, f"input: expected {cdt} [{m}, {c_in}]"
+    for p in packeds:
+        assert p.dtype == torch.uint8 and p.numel() * 2 == n_out * k_in, "packed: uint8 holding N * K / 2 bytes"
+    assert state_dtype in (torch.bfloat16, torch.float16, torch.float32), f"state dtype: 16/32-bit float, got {state_dtype}"
+    twice = cdt == torch.bfloat16 and state_dtype == torch.float16
+    out_ok = (cdt, torch.float32, torch.float16) if cdt == torch.bfloat16 else (cdt, torch.float32)
+    assert out_dtype in out_ok, f"out_dtype: one of {out_ok}, got {out_dtype}"
+    ex = twice or (cdt == torch.bfloat16 and out_dtype == torch.float16)
+    assert not (ex and row_scales), "row scales need a bf16 or fp32 state and a bf16 or fp32 output"
+    assert not biases or len(biases) == n, "one bias (or None) per problem"
+    for b in biases:
+        if b is not None:
+            assert not is_bwd and b.numel() == n_out, "bias: N elements, forward only"
+    assert len(us) == len(vs) and (not us or len(us) == n), "LoRA: one U and one V per problem, or none"
+    r = us[0].shape[1] if us else 0
+    for u, v in zip(us, vs):
+        assert u.dim() == 2 and u.shape == (m, r) and u.dtype == cdt, f"U: expected {cdt} [{m}, {r}]"
+        assert v.shape == ((r, k_in) if is_bwd else (n_out, r)) and v.dtype == cdt, "V: lora_A [r, K] (dX) or lora_B [N, r]"
+    n_outs = 1 if is_bwd else n
+    assert len(outs) == n_outs, f"outs: {n_outs} tensors"
+    for o in outs:
+        assert o.shape == (m, f_out) and o.stride(1) == 1 and o.dtype == out_dtype, f"out: {out_dtype} [{m}, {f_out}] rows"
+    assert not row_scales or len(row_scales) == n, "one row scale (or None) per problem"
+    for sc in row_scales:
+        if sc is not None:
+            assert sc.shape == (n_out,) and sc.dtype == torch.float32 and sc.device == dev, "row scale: fp32 [N] on the GPU"
+    assert w_scratch is None or (not row_scales and w_scratch.dtype == torch.uint8 and w_scratch.device == dev)
+    return dev, m, r, c_in, f_out, cdt, twice, ex
+
+
+@torch.library.custom_op("qlora_b200::nf4_linear_group", mutates_args=("outs", "w_scratch"))
+def nf4_linear_group(is_bwd: bool, inputs: list[Tensor], packeds: list[Tensor], absmax: list[Tensor],
+                     code2: list[Optional[Tensor]], absmax2: list[Optional[Tensor]], offset: list[Optional[Tensor]],
+                     n_out: int, k_in: int, state_dtype: torch.dtype, biases: list[Optional[Tensor]], us: list[Tensor],
+                     vs: list[Tensor], outs: list[Tensor], out_dtype: torch.dtype, row_scales: list[Optional[Tensor]],
+                     w_scratch: Optional[Tensor], return_scratch: bool) -> Tensor:
+    """`functional.nf4_linear_group` on the state's tensors, writing its results into `outs` (one per problem forward, one
+    for the dX).  Empty lists stand for None (`biases`, `us` / `vs`, `row_scales`: a non-empty `row_scales` selects the
+    row-scaled launch even when every entry is None).  The outputs are lent rather than returned because torch cannot
+    functionalize an op that both mutates a list and returns one.  A lent `w_scratch` is declared mutated too: a call off
+    the scratch path uses it as its split-K workspace.
+
+    Returns the scratch: with `return_scratch`, the workspace when the call left its bf16 weight copies there, or with
+    `w_scratch` lent, a one-byte tensor when the GEMM read the lent copies; an empty tensor otherwise."""
+    dev, m, r, c_in, f_out, cdt, twice, ex = _check_group(is_bwd, inputs, packeds, absmax, code2, absmax2, offset, n_out, k_in,
+                                                          state_dtype, biases, us, vs, outs, out_dtype, row_scales, w_scratch)
+    n = len(packeds)
+    n_outs = 1 if is_bwd else n
+    none = torch.empty(0, dtype=torch.uint8, device=dev)
+    if m == 0:
+        return none
+    lib = _lib.load()
+    keep = []  # tensors that must outlive the launch call
+    probs = (_lib.Nf4Problem * n)()
+
+    def _rowmajor(t, cols):
+        if t.stride(1) != 1 or (t.stride(0) % 8) or t.stride(0) < cols or (t.data_ptr() % 16):
+            t = t.contiguous()
+            keep.append(t)
+        return t
+
+    for i in range(n):
+        x = _rowmajor(inputs[i], c_in)
+        packed = packeds[i]
+        if not packed.is_contiguous():
+            packed = packed.contiguous()
+            keep.append(packed)
+        pr = probs[i]
+        pr.inp, pr.ld_in = x.data_ptr(), x.stride(0)
+        pr.packed = packed.data_ptr()
+        if code2[i] is not None:
+            pr.absmax_u8, pr.code256, pr.absmax2, pr.offset = (absmax[i].data_ptr(), code2[i].data_ptr(), absmax2[i].data_ptr(),
+                                                               offset[i].data_ptr())
+        else:
+            pr.absmax_f32 = absmax[i].data_ptr()
+        b = biases[i] if biases else None
+        if b is not None:
+            b = b.to(cdt).contiguous()
+            keep.append(b)
+            pr.bias = b.data_ptr()
+        if r:
+            u = _rowmajor(us[i], r)
+            v = vs[i]
+            if not v.is_contiguous():
+                v = v.contiguous()
+                keep.append(v)
+            pr.U, pr.ld_u, pr.V = u.data_ptr(), u.stride(0), v.data_ptr()
+        if i < n_outs:
+            o = outs[i]
+            pr.out, pr.ld_out = o.data_ptr(), o.stride(0)
+    scales = None
+    if row_scales:
+        scales = (ct.c_void_p * n)()
+        for i, sc in enumerate(row_scales):
+            if sc is None:
+                continue
+            if not sc.is_contiguous():
+                sc = sc.contiguous()
+                keep.append(sc)
+            scales[i] = sc.data_ptr()
+    ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
+    # training token counts under bf16 compute (bf16 or fp32 state, bf16 or fp32 output, no row scale): each W is dequantized
+    # once into a bf16 scratch that a TMA-fed GEMM reads; one dequantize launch per problem precedes the GEMM, unless the
+    # caller passes back the scratch of an earlier call (w_scratch)
+    scratch = (lib.qb200_nf4_linear_scratch_size(n, m, n_out, k_in, int(is_bwd))
+               if cdt == torch.bfloat16 and not ex and scales is None else 0)
+    ws_bytes = max(ws_bytes, scratch)
+    if w_scratch is not None:
+        ws, ws_bytes = w_scratch, w_scratch.numel()
+    else:
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
+    w_in_ws = ct.c_int(int(w_scratch is not None))
+    what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
+            + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else "")
+            + ("_sf16" if twice else "") + ("_of16" if ex and out_dtype == torch.float16 else ""))
+    with torch.cuda.device(dev):
+        ev = F._event_begin()
+        if scales is None:
+            rc = lib.qb200_nf4_linear_group_reuse(int(is_bwd), DTYPE_CODE[cdt], DTYPE_CODE[state_dtype], n, ct.addressof(probs), r,
+                                                  m, n_out, k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, ct.byref(w_in_ws),
+                                                  stream_ptr(dev))
+        else:
+            rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), DTYPE_CODE[cdt], n, ct.addressof(probs), ct.addressof(scales), r, m,
+                                                  n_out, k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
+        check(rc, what)
+        F._event_end(what, m * n, n_out, k_in, ev)
+    if w_in_ws.value and w_scratch is None:
+        F.LAUNCH_COUNTER[0] += n   # the dequantize launches that wrote the scratch
+    if return_scratch and w_in_ws.value:
+        none = ws if w_scratch is None else torch.zeros(1, dtype=torch.uint8, device=dev)
+    return none
+
+
+@nf4_linear_group.register_fake
+def _(is_bwd, inputs, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, us, vs, outs, out_dtype,
+      row_scales, w_scratch, return_scratch):
+    dev, m, r, c_in, f_out, cdt, twice, ex = _check_group(is_bwd, inputs, packeds, absmax, code2, absmax2, offset, n_out, k_in,
+                                                          state_dtype, biases, us, vs, outs, out_dtype, row_scales, w_scratch)
+    # whether the call leaves its weights in the workspace is decided by the library at run time
+    size = torch.library.get_ctx().new_dynamic_size() if return_scratch else 0
+    return inputs[0].new_empty((size,), dtype=torch.uint8)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the lora_A projection U = scale * x . A^T
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _check_lora_project(x2d: Tensor, lora_a: Tensor) -> None:
+    _device(x2d, lora_a)
+    assert x2d.dim() == 2 and lora_a.dim() == 2 and lora_a.shape[1] == x2d.shape[1], "x2d [M, K] and lora_a [r, K]"
+    assert lora_a.dtype == x2d.dtype, "x2d and lora_a of one dtype"
+
+
+@torch.library.custom_op("qlora_b200::lora_project", mutates_args=())
+def lora_project(x2d: Tensor, lora_a: Tensor, scale: float) -> Tensor:
+    """U[M, r] = scale * x2d . lora_a^T.  A decode step (1..16 tokens, bf16 or fp16, K a multiple of 8, contiguous A) takes
+    the library's one-launch projection (`qb200_lora_project` / `_typed`), which chains with the skinny kernel by
+    programmatic dependent launch; every other call is one cuBLAS GEMM with the scale as its alpha.  The choice is made
+    here, at run time, so that a graph traced with a symbolic token count serves both."""
+    _check_lora_project(x2d, lora_a)
+    dev = x2d.device
+    m, k = x2d.shape
+    r = lora_a.shape[0]
+    if not (1 <= m <= F.LORA_PROJECT_MAX_TOKENS and k % 8 == 0 and x2d.dtype in (torch.bfloat16, torch.float16)
+            and lora_a.is_contiguous()):
+        u = torch.empty((m, r), dtype=x2d.dtype, device=dev)
+        return torch.addmm(u, x2d, lora_a.t(), beta=0.0, alpha=scale, out=u)
+    if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k or x2d.data_ptr() % 16:
+        x2d = x2d.contiguous()
+    if not lora_a.is_contiguous() or lora_a.data_ptr() % 16:
+        lora_a = lora_a.contiguous()
+    u = torch.empty((m, r), dtype=x2d.dtype, device=dev)
+    F.LAUNCH_COUNTER[0] += 1
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        if x2d.dtype == torch.float16:
+            rc = lib.qb200_lora_project_typed(DTYPE_CODE[torch.float16], ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u),
+                                              r, m, k, r, stream_ptr(dev))
+        else:
+            rc = lib.qb200_lora_project(ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u), r, m, k, r, stream_ptr(dev))
+        check(rc, "lora_project")
+    return u
+
+
+@lora_project.register_fake
+def _(x2d, lora_a, scale):
+    _check_lora_project(x2d, lora_a)
+    return x2d.new_empty((x2d.shape[0], lora_a.shape[0]))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# NF4 and 8-bit blockwise (de)quantization
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _check_dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, out):
+    _device(packed, absmax, code2, absmax2, offset, out)
+    _check_state(absmax, code2, absmax2, offset)
+    _check_blocksize(blocksize)
+    if code2 is not None:
+        _check_blocksize(blocksize2)
+    assert packed.dtype == torch.uint8 and packed.is_contiguous(), "packed: contiguous uint8"
+    if out.dtype not in DTYPE_CODE:
+        raise ValueError(f"Blockwise quantization only supports 16/32-bit floats, but got {out.dtype}")
+    assert out.is_contiguous(), "out must be contiguous"
+
+
+def _dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, out) -> None:
+    dev = out.device
+    lib = _lib.load()
+    F.LAUNCH_COUNTER[0] += 1
+    with torch.cuda.device(dev):
+        if code2 is not None:
+            check(lib.qb200_dequantize_nf4_nested(ptr(packed), ptr(absmax), ptr(code2), ptr(absmax2), ptr(offset), out.numel(),
+                                                  blocksize, blocksize2, ptr(out), DTYPE_CODE[out.dtype], stream_ptr(dev)),
+                  "dequantize_4bit")
+        else:
+            check(lib.qb200_dequantize_nf4(ptr(packed), ptr(absmax), out.numel(), blocksize, ptr(out), DTYPE_CODE[out.dtype],
+                                           stream_ptr(dev)), "dequantize_4bit")
+
+
+@torch.library.custom_op("qlora_b200::dequantize_nf4", mutates_args=("out",))
+def dequantize_nf4(packed: Tensor, absmax: Tensor, code2: Optional[Tensor], absmax2: Optional[Tensor], offset: Optional[Tensor],
+                   blocksize: int, blocksize2: int, out: Tensor) -> None:
+    """out = the NF4 weights of `packed` (K4; for a nested state K3 + offset add + K4 as one kernel), in out's dtype."""
+    _check_dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, out)
+    _dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, out)
+
+
+@dequantize_nf4.register_fake
+def _(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, out):
+    _check_dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, out)
+
+
+def _check_quantize_nf4(A, blocksize, out, absmax):
+    _device(A, out, absmax)
+    if A.dtype not in DTYPE_CODE:
+        raise ValueError(f"Blockwise quantization only supports 16/32-bit floats, but got {A.dtype}")
+    _check_blocksize(blocksize)
+    assert A.is_contiguous(), "A must be contiguous"
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.numel() * 2 >= A.numel(), "out: contiguous uint8, n/2 bytes"
+    assert absmax.dtype == torch.float32 and absmax.is_contiguous() and absmax.numel() * blocksize >= A.numel(), \
+        "absmax: contiguous fp32, one per block"
+
+
+@torch.library.custom_op("qlora_b200::quantize_nf4", mutates_args=("out", "absmax"))
+def quantize_nf4(A: Tensor, blocksize: int, out: Tensor, absmax: Tensor) -> None:
+    """NF4 blockwise quantization of A (K1): packed codes into `out`, the fp32 absmax of every block into `absmax`."""
+    _check_quantize_nf4(A, blocksize, out, absmax)
+    dev = A.device
+    with torch.cuda.device(dev):
+        check(_lib.load().qb200_quantize_nf4(ptr(A), DTYPE_CODE[A.dtype], A.numel(), blocksize, ptr(out), ptr(absmax),
+                                             stream_ptr(dev)), "quantize_4bit")
+
+
+@quantize_nf4.register_fake
+def _(A, blocksize, out, absmax):
+    _check_quantize_nf4(A, blocksize, out, absmax)
+
+
+def _check_blockwise(code, A, absmax, blocksize, out, quantize):
+    _device(code, A, absmax, out)
+    _check_blocksize(blocksize)
+    assert code.dtype == torch.float32 and code.is_contiguous(), "code: contiguous fp32"
+    assert A.is_contiguous() and out.is_contiguous() and A.numel() == out.numel(), "A and out: contiguous, of one size"
+    assert absmax.dtype == torch.float32 and absmax.is_contiguous() and absmax.numel() * blocksize >= A.numel(), \
+        "absmax: contiguous fp32, one per block"
+    src, dst = (A, out) if quantize else (out, A)
+    assert src.dtype == torch.float32 and dst.dtype == torch.uint8, "fp32 values, uint8 codes"
+
+
+@torch.library.custom_op("qlora_b200::quantize_blockwise", mutates_args=("out", "absmax"))
+def quantize_blockwise(code: Tensor, A: Tensor, blocksize: int, out: Tensor, absmax: Tensor) -> None:
+    """8-bit blockwise quantization of fp32 A against a 256-entry codebook (K2)."""
+    _check_blockwise(code, A, absmax, blocksize, out, True)
+    dev = A.device
+    with torch.cuda.device(dev):
+        check(_lib.load().qb200_quantize_blockwise_8bit(ptr(code), ptr(A), A.numel(), blocksize, ptr(out), ptr(absmax),
+                                                        stream_ptr(dev)), "quantize_blockwise")
+
+
+@quantize_blockwise.register_fake
+def _(code, A, blocksize, out, absmax):
+    _check_blockwise(code, A, absmax, blocksize, out, True)
+
+
+@torch.library.custom_op("qlora_b200::dequantize_blockwise", mutates_args=("out",))
+def dequantize_blockwise(code: Tensor, A: Tensor, absmax: Tensor, blocksize: int, out: Tensor) -> None:
+    """8-bit blockwise dequantization (K3): out[i] = code[A[i]] * absmax[i // blocksize], fp32."""
+    _check_blockwise(code, A, absmax, blocksize, out, False)
+    dev = A.device
+    with torch.cuda.device(dev):
+        check(_lib.load().qb200_dequantize_blockwise_8bit(ptr(code), ptr(A), ptr(absmax), A.numel(), blocksize, ptr(out),
+                                                          stream_ptr(dev)), "dequantize_blockwise")
+
+
+@dequantize_blockwise.register_fake
+def _(code, A, absmax, blocksize, out):
+    _check_blockwise(code, A, absmax, blocksize, out, False)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# DoRA: the squared row norms of a frozen NF4 weight
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _check_row_norm2(packed, absmax, code2, absmax2, offset, n_out, k_in, dtype, blocksize, blocksize2):
+    _check_dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, packed.new_empty(0, dtype=dtype))
+    assert packed.numel() * 2 == n_out * k_in, "packed: N * K / 2 bytes"
+
+
+@torch.library.custom_op("qlora_b200::weight_row_norm2", mutates_args=())
+def weight_row_norm2(packed: Tensor, absmax: Tensor, code2: Optional[Tensor], absmax2: Optional[Tensor], offset: Optional[Tensor],
+                     n_out: int, k_in: int, dtype: torch.dtype, blocksize: int, blocksize2: int) -> Tensor:
+    """||W_f||^2 for every row f: the weight `dequantize_4bit` returns in `dtype`, squared and summed in fp32; fp32 [N]."""
+    _check_row_norm2(packed, absmax, code2, absmax2, offset, n_out, k_in, dtype, blocksize, blocksize2)
+    w = torch.empty((n_out, k_in), dtype=dtype, device=packed.device)
+    _dequantize_nf4(packed, absmax, code2, absmax2, offset, blocksize, blocksize2, w)
+    norm2 = torch.empty(n_out, dtype=torch.float32, device=w.device)
+    for r0 in range(0, n_out, 2048):                       # fp32 copies of 2048 rows at a time
+        norm2[r0:r0 + 2048] = w[r0:r0 + 2048].float().square().sum(1)
+    return norm2
+
+
+@weight_row_norm2.register_fake
+def _(packed, absmax, code2, absmax2, offset, n_out, k_in, dtype, blocksize, blocksize2):
+    _check_row_norm2(packed, absmax, code2, absmax2, offset, n_out, k_in, dtype, blocksize, blocksize2)
+    return packed.new_empty((n_out,), dtype=torch.float32)

@@ -74,7 +74,8 @@ class MatMul4Bit(torch.autograd.Function):
         else:
             output = torch.nn.functional.linear(A, _unfused_weight(B, quant_state, A.dtype).t(), bias)
         kept = F.scratch_to_save(scratch, ctx.needs_input_grad[0])   # a checkpoint recompute's W copy, for the dX launch
-        ctx.save_for_backward(*kept)
+        # only the PACKED weight is kept for backward (no bf16 W is saved)
+        ctx.save_for_backward(*([B] if any(ctx.needs_input_grad[:2]) else []), *kept)
         ctx.kept_scratch = bool(kept)
         if out is not None:
             out.copy_(output)
@@ -83,10 +84,6 @@ class MatMul4Bit(torch.autograd.Function):
         ctx.state = quant_state
         ctx.fused, ctx.cdt = fused, cdt
         ctx.dtype_A, ctx.dtype_B, ctx.dtype_bias = A.dtype, B.dtype, None if bias is None else bias.dtype
-        if any(ctx.needs_input_grad[:2]):
-            ctx.tensors = (None, B)  # only the PACKED weight is kept for backward (no bf16 W is saved)
-        else:
-            ctx.tensors = (None, None)
         return output
 
     @staticmethod
@@ -95,14 +92,15 @@ class MatMul4Bit(torch.autograd.Function):
             bias_grad = None if ctx.bias is None else torch.zeros_like(ctx.bias)
             return torch.zeros_like(ctx.A), torch.zeros_like(ctx.B), None, bias_grad, None, None
         req_gradA, _, _, req_gradBias = ctx.needs_input_grad[:4]
-        _, B = ctx.tensors
         grad_A, grad_B, grad_bias = None, None, None
         if req_gradBias:
             # sum over every leading dim (upstream sums dim 0 only, which is wrong for 3-D inputs)
             grad_bias = grad_output.reshape(-1, grad_output.shape[-1]).sum(0, dtype=ctx.dtype_bias)
         if req_gradA:
+            saved = ctx.saved_tensors
+            B = saved[0]
             if ctx.fused and (ctx.io_dtype is not None or grad_output.dtype == ctx.cdt):
-                scratch = F.saved_scratch(ctx.saved_tensors) if ctx.kept_scratch else None
+                scratch = F.saved_scratch(saved) if ctx.kept_scratch else None
                 dx = F.nf4_linear_group(True, [F.as_compute_2d(grad_output, ctx.cdt)], [B], [ctx.state],
                                         out_dtype=F.out_dtype_for(ctx.dtype_A, ctx.cdt), w_scratch=scratch)
                 grad_A = dx.view(*grad_output.shape[:-1], ctx.state.shape[1])

@@ -14,7 +14,6 @@ in oracle/ and is test infrastructure).
 """
 from __future__ import annotations
 
-import ctypes as ct
 import json
 from math import prod
 from typing import Any, Optional
@@ -22,8 +21,8 @@ from typing import Any, Optional
 import torch
 from torch import Tensor
 
-from . import _lib
-from ._lib import DTYPE_CODE, check, ptr, stream_ptr
+from . import _lib, _ops
+from ._lib import DTYPE_CODE, check, ptr, stream_ptr  # noqa: F401  (ptr, stream_ptr: used by callers of F)
 
 name2qmap: dict[str, Tensor] = {}
 
@@ -235,25 +234,6 @@ class QuantState:
     __hash__ = None  # mutable container
 
 
-def _require_cuda(*tensors: Optional[Tensor]) -> torch.device:
-    dev = None
-    for t in tensors:
-        if t is None:
-            continue
-        if not t.is_cuda:
-            raise RuntimeError(
-                "qlora_b200 ops run on CUDA tensors only (H100-native kernels, no CPU fallback); "
-                f"got a tensor on {t.device}"
-            )
-        if dev is None:
-            dev = t.device
-        elif t.device != dev:
-            raise RuntimeError(f"all tensors must be on the same GPU, found {dev} and {t.device}")
-    if dev is None:
-        raise RuntimeError("no tensors given")
-    return dev
-
-
 def _default_code(device) -> Tensor:
     if "dynamic" not in name2qmap:
         name2qmap["dynamic"] = create_dynamic_map()
@@ -266,13 +246,11 @@ def _default_code(device) -> Tensor:
 def quantize_blockwise(A: Tensor, code: Optional[Tensor] = None, absmax: Optional[Tensor] = None, out: Optional[Tensor] = None,
                        blocksize: int = 4096, nested: bool = False) -> tuple[Tensor, QuantState]:
     """8-bit blockwise quantization against a 256-entry codebook (K2; used for nested absmax)."""
-    dev = _require_cuda(A)
-    lib = _lib.load()
+    dev = _ops._device(A)
     if code is None:
         code = _default_code(dev)
     code = code.to(device=dev, dtype=torch.float32).contiguous()
-    if blocksize not in (4096, 2048, 1024, 512, 256, 128, 64):
-        raise ValueError(f"blocksize {blocksize} not in (4096, 2048, 1024, 512, 256, 128, 64)")
+    _ops._check_blocksize(blocksize)
     n = A.numel()
     blocks = -(n // -blocksize)
     if absmax is None:
@@ -282,9 +260,7 @@ def quantize_blockwise(A: Tensor, code: Optional[Tensor] = None, absmax: Optiona
     elif not out.is_contiguous() or out.dtype != torch.uint8 or out.numel() != n:
         raise ValueError("quantize_blockwise: `out` must be a contiguous uint8 tensor with A.numel() elements")
     A32 = A.contiguous().float()  # widening is exact; the kernel computes in fp32 like upstream
-    with torch.cuda.device(dev):
-        check(lib.qb200_quantize_blockwise_8bit(ptr(code), ptr(A32), n, blocksize, ptr(out), ptr(absmax), stream_ptr(dev)),
-              "quantize_blockwise")
+    _ops.quantize_blockwise(code, A32, blocksize, out, absmax)
     if nested:
         offset = absmax.mean()
         absmax -= offset
@@ -300,8 +276,7 @@ def dequantize_blockwise(A: Tensor, quant_state: Optional[QuantState] = None, ab
                          nested: bool = False) -> Tensor:
     """8-bit blockwise dequantization (K3): out[i] = code[A[i]] * absmax[i // blocksize]."""
     assert quant_state is not None or absmax is not None
-    dev = _require_cuda(A)
-    lib = _lib.load()
+    dev = _ops._device(A)
     if quant_state is None:
         if code is None:
             code = _default_code(dev)
@@ -312,13 +287,10 @@ def dequantize_blockwise(A: Tensor, quant_state: Optional[QuantState] = None, ab
         absmax = absmax + quant_state.offset
     if absmax.dtype != torch.float32:
         absmax = absmax.float()
-    if quant_state.blocksize not in (4096, 2048, 1024, 512, 256, 128, 64):
-        raise ValueError(f"blocksize {quant_state.blocksize} not in (4096, 2048, 1024, 512, 256, 128, 64)")
+    _ops._check_blocksize(quant_state.blocksize)
     code32 = quant_state.code.to(device=dev, dtype=torch.float32).contiguous()
     out32 = out if (out is not None and out.dtype == torch.float32) else torch.empty(A.shape, dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        check(lib.qb200_dequantize_blockwise_8bit(ptr(code32), ptr(A.contiguous()), ptr(absmax.contiguous()), A.numel(),
-                                                  quant_state.blocksize, ptr(out32), stream_ptr(dev)), "dequantize_blockwise")
+    _ops.dequantize_blockwise(code32, A.contiguous(), absmax.contiguous(), quant_state.blocksize, out32)
     target = quant_state.dtype if quant_state.dtype is not None else torch.float32
     if out is not None and out is not out32:
         out.copy_(out32)
@@ -334,16 +306,14 @@ def quantize_4bit(A: Tensor, absmax: Optional[Tensor] = None, out: Optional[Tens
     nibble; absmax per `blocksize` flat elements; with `compress_statistics` the fp32 absmax is
     itself quantized to 8 bits in blocks of 256 after subtracting its mean (double quantization).
     """
-    dev = _require_cuda(A)
-    lib = _lib.load()
+    dev = _ops._device(A)
     if quant_type not in ("fp4", "nf4"):
         raise NotImplementedError(f"4-bit quantization data type {quant_type} is not implemented.")
     if quant_type == "fp4":
         raise NotImplementedError("quant_type='fp4' is outside this build's scope (NF4 only; SURVEY.md 2.2)")
     if A.dtype not in DTYPE_CODE:
         raise ValueError(f"Blockwise quantization only supports 16/32-bit floats, but got {A.dtype}")
-    if blocksize not in (4096, 2048, 1024, 512, 256, 128, 64):
-        raise ValueError(f"blocksize {blocksize} not in (4096, 2048, 1024, 512, 256, 128, 64)")
+    _ops._check_blocksize(blocksize)
     if quant_storage != torch.uint8:
         raise NotImplementedError("quant_storage other than torch.uint8 is not implemented")
     n = A.numel()
@@ -354,9 +324,7 @@ def quantize_4bit(A: Tensor, absmax: Optional[Tensor] = None, out: Optional[Tens
     if out is None:
         out = torch.empty(((n + 1) // 2, 1), dtype=torch.uint8, device=dev)
     A = A.contiguous()
-    with torch.cuda.device(dev):
-        check(lib.qb200_quantize_nf4(ptr(A), DTYPE_CODE[A.dtype], n, blocksize, ptr(out), ptr(absmax), stream_ptr(dev)),
-              "quantize_4bit")
+    _ops.quantize_nf4(A, blocksize, out, absmax)
     code = get_4bit_type(quant_type, device=dev)
     if compress_statistics:
         offset = absmax.mean()  # reduction order = torch's, exactly as the reference computes it
@@ -377,8 +345,7 @@ def dequantize_4bit(A: Tensor, quant_state: Optional[QuantState] = None, absmax:
     Returns a tensor of `quant_state.shape` / `quant_state.dtype`; like upstream, if `A` is the
     transposed `[1, n/2]` view that `matmul_4bit` passes, the result is returned transposed.
     """
-    dev = _require_cuda(A)
-    lib = _lib.load()
+    dev = _ops._device(A)
     if quant_state is None:
         assert absmax is not None and out is not None
         if quant_type != "nf4":
@@ -386,26 +353,13 @@ def dequantize_4bit(A: Tensor, quant_state: Optional[QuantState] = None, absmax:
         quant_state = QuantState(absmax=absmax, shape=out.shape, dtype=out.dtype, blocksize=blocksize, quant_type=quant_type)
     if quant_state.quant_type != "nf4":
         raise NotImplementedError(f"4-bit quantization data type {quant_state.quant_type} is not implemented.")
-    if quant_state.blocksize not in (4096, 2048, 1024, 512, 256, 128, 64):
-        raise ValueError(f"blocksize {quant_state.blocksize} not in (4096, 2048, 1024, 512, 256, 128, 64)")
+    _ops._check_blocksize(quant_state.blocksize)
     if out is None:
         out = torch.empty(quant_state.shape, dtype=quant_state.dtype, device=dev)
     if out.dtype not in DTYPE_CODE:
         raise ValueError(f"Blockwise quantization only supports 16/32-bit floats, but got {out.dtype}")
-    n = out.numel()
     packed = A if A.is_contiguous() else A.contiguous()  # the [1, n/2] .t() view of a [n/2, 1] tensor is contiguous
-    LAUNCH_COUNTER[0] += 1
-    with torch.cuda.device(dev):
-        if quant_state.nested:
-            s2 = quant_state.state2
-            _state_tensors(quant_state, dev)  # u8 codes, fp32 code / absmax2 / offset, contiguous, on this device
-            check(lib.qb200_dequantize_nf4_nested(ptr(packed), ptr(quant_state.absmax), ptr(s2.code), ptr(s2.absmax),
-                                                  ptr(quant_state.offset), n, quant_state.blocksize, s2.blocksize,
-                                                  ptr(out), DTYPE_CODE[out.dtype], stream_ptr(dev)), "dequantize_4bit")
-        else:
-            am = _checked(quant_state.absmax, torch.float32, dev, "absmax")
-            check(lib.qb200_dequantize_nf4(ptr(packed), ptr(am), n, quant_state.blocksize, ptr(out), DTYPE_CODE[out.dtype],
-                                           stream_ptr(dev)), "dequantize_4bit")
+    _ops.dequantize_nf4(packed, *_state_args(quant_state, dev), out)
     is_transposed = A.shape[0] == 1
     return out.t() if is_transposed else out
 
@@ -497,26 +451,37 @@ def _checked(t: Tensor, dtype: torch.dtype, dev: torch.device, what: str) -> Ten
 
 def _state_tensors(qs: QuantState, dev: torch.device):
     """(absmax_u8, code256, absmax2, offset, absmax_f32) validated for the fused kernel (ADVICE r1: dtype / device /
-    contiguity are checked, never assumed)."""
+    contiguity are checked, never assumed).  Only converted copies are written back, so a state the kernels can read as it
+    is stays untouched (what lets torch.compile trace this without a side effect)."""
     if qs.nested:
         s2 = qs.state2
-        qs.absmax = _checked(qs.absmax, torch.uint8, dev, "absmax")
-        s2.code = _checked(s2.code, torch.float32, dev, "state2.code")
-        s2.absmax = _checked(s2.absmax, torch.float32, dev, "state2.absmax")
-        qs.offset = _checked(qs.offset, torch.float32, dev, "offset")
+        for obj, name, dtype, what in ((qs, "absmax", torch.uint8, "absmax"), (s2, "code", torch.float32, "state2.code"),
+                                       (s2, "absmax", torch.float32, "state2.absmax"), (qs, "offset", torch.float32, "offset")):
+            t = getattr(obj, name)
+            c = _checked(t, dtype, dev, what)
+            if c is not t:
+                setattr(obj, name, c)
         return qs.absmax, s2.code, s2.absmax, qs.offset, None
-    qs.absmax = _checked(qs.absmax, torch.float32, dev, "absmax")
+    a = _checked(qs.absmax, torch.float32, dev, "absmax")
+    if a is not qs.absmax:
+        qs.absmax = a
     return None, None, None, None, qs.absmax
 
 
-_F16_CODE = DTYPE_CODE[torch.float16]
+def _state_args(qs: QuantState, dev: torch.device):
+    """The state as the dequantize ops take it: (absmax, code2, absmax2, offset, blocksize, blocksize2)."""
+    if qs.nested:
+        a_u8, code, a2, off, _ = _state_tensors(qs, dev)
+        return a_u8, code, a2, off, qs.blocksize, qs.state2.blocksize
+    return _checked(qs.absmax, torch.float32, dev, "absmax"), None, None, None, qs.blocksize, 0
+
 
 
 def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None, vs=None, outs=None,
                      out_dtype: Optional[torch.dtype] = None, row_scales=None, w_scratch: Optional[Tensor] = None,
                      return_scratch: bool = False):
     """1..3 `Linear4bit` of one shape in ONE launch of the fused kernel (`qb200_nf4_linear_group_reuse`, or
-    `qb200_nf4_linear_group_typed` with row scales).
+    `qb200_nf4_linear_group_typed` with row scales), through the `qlora_b200::nf4_linear_group` op.
 
     The inputs' dtype (bf16 or fp16) is the compute dtype: U / V / bias are of it too and `out_dtype` is it (the default) or
     fp32 (the result rounded to it, widened); under bf16 compute it may also be fp16 (the bf16-rounded result rounded to
@@ -533,120 +498,35 @@ def nf4_linear_group(is_bwd: bool, inputs, packeds, states, biases=None, us=None
     Training token counts (the scratch path) dequantize every W_p into a bf16 scratch that the GEMM reads.  return_scratch:
     also return that scratch, or None when the call left no W_p there: (result, scratch).  w_scratch: a scratch returned by
     an earlier call on the same packed weights and states, in the same order; a call that takes the scratch path then skips
-    the dequantize launches and reads it.
+    the dequantize launches and reads it.  Under torch.compile no scratch is returned (None): whether a call leaves one is
+    decided at run time, and a graph cannot branch on it.
     """
     n = len(states)
     assert 1 <= n <= 3 and len(inputs) == n and len(packeds) == n
-    dev = _require_cuda(*inputs, *packeds)
-    lib = _lib.load()
+    dev = _ops._device(*inputs, *packeds)
     n_out, k_in = states[0].shape
     for qs in states:
         assert tuple(qs.shape) == (n_out, k_in), "grouped problems must share their weight shape"
-    c_in, f_out = (n_out, k_in) if is_bwd else (k_in, n_out)
-    m = inputs[0].shape[0]
-    r = 0 if us is None else us[0].shape[1]
-    n_outs = 1 if is_bwd else n
     cdt = inputs[0].dtype
-    assert cdt in (torch.bfloat16, torch.float16), f"inputs: bf16 or fp16, got {cdt}"
     twice = double_rounded(states[0], cdt)
     assert all(double_rounded(qs, cdt) == twice for qs in states), "grouped problems must share the rounding of their weights"
-    sdt = states[0].dtype
+    sts = [_state_tensors(qs, dev) for qs in states]
+    return_scratch_op = return_scratch and not torch.compiler.is_compiling()
     out_dtype = cdt if out_dtype is None else out_dtype
-    out_ok = (cdt, torch.float32, torch.float16) if cdt == torch.bfloat16 else (cdt, torch.float32)
-    assert out_dtype in out_ok, f"out_dtype: one of {out_ok}, got {out_dtype}"
-    # bf16 compute over an fp16 state or with an fp16 output: the fused kernel at every token count, no row scales
-    ex = twice or (cdt == torch.bfloat16 and out_dtype == torch.float16)
-    assert not (ex and row_scales is not None), "row scales need a bf16 or fp32 state and a bf16 or fp32 output"
     if outs is None:
-        outs = [torch.empty((m, f_out), dtype=out_dtype, device=dev) for _ in range(n_outs)]
-    if m == 0:
-        return (outs[0] if is_bwd else outs, None) if return_scratch else (outs[0] if is_bwd else outs)
-    keep = []  # tensors that must outlive the launch call
-    probs = (_lib.Nf4Problem * n)()
-
-    def _rowmajor(t, cols, what):
-        assert t.dim() == 2 and t.shape == (m, cols) and t.dtype == cdt, f"{what}: expected {cdt} [{m}, {cols}]"
-        if t.stride(1) != 1 or (t.stride(0) % 8) or t.stride(0) < cols or (t.data_ptr() % 16):
-            t = t.contiguous()
-            keep.append(t)
-        return t
-
-    for i in range(n):
-        x = _rowmajor(inputs[i], c_in, "input")
-        a_u8, code, a2, off, a_f32 = _state_tensors(states[i], dev)
-        packed = packeds[i]
-        if not packed.is_contiguous():
-            packed = packed.contiguous()
-            keep.append(packed)
-        pr = probs[i]
-        pr.inp, pr.ld_in = x.data_ptr(), x.stride(0)
-        pr.packed = packed.data_ptr()
-        pr.absmax_u8 = None if a_u8 is None else a_u8.data_ptr()
-        pr.code256 = None if code is None else code.data_ptr()
-        pr.absmax2 = None if a2 is None else a2.data_ptr()
-        pr.offset = None if off is None else off.data_ptr()
-        pr.absmax_f32 = None if a_f32 is None else a_f32.data_ptr()
-        b = None if biases is None else biases[i]
-        if b is not None:
-            assert not is_bwd and b.numel() == n_out
-            b = b.to(cdt).contiguous()
-            keep.append(b)
-            pr.bias = b.data_ptr()
-        if r:
-            u = _rowmajor(us[i], r, "U")
-            v = vs[i]
-            assert v.shape == ((r, k_in) if is_bwd else (n_out, r)) and v.dtype == cdt
-            if not v.is_contiguous():
-                v = v.contiguous()
-                keep.append(v)
-            pr.U, pr.ld_u, pr.V = u.data_ptr(), u.stride(0), v.data_ptr()
-        if i < n_outs:
-            o = outs[i]
-            assert o.shape == (m, f_out) and o.stride(1) == 1 and o.dtype == out_dtype
-            pr.out, pr.ld_out = o.data_ptr(), o.stride(0)
-    scales = None
-    if row_scales is not None:
-        assert len(row_scales) == n
-        scales = (ct.c_void_p * n)()
-        for i, sc in enumerate(row_scales):
-            if sc is None:
-                continue
-            assert sc.shape == (n_out,) and sc.dtype == torch.float32 and sc.device == dev, "row scale: fp32 [N] on the GPU"
-            if not sc.is_contiguous():
-                sc = sc.contiguous()
-                keep.append(sc)
-            scales[i] = sc.data_ptr()
-    ws_bytes = lib.qb200_nf4_linear_workspace_size(m, n_out, k_in, int(is_bwd)) if n == 1 else 0
-    # training token counts under bf16 compute (bf16 or fp32 state, bf16 or fp32 output, no row scale): each W is dequantized
-    # once into a bf16 scratch that a TMA-fed GEMM reads; one dequantize launch per problem precedes the GEMM, unless the
-    # caller passes back the scratch of an earlier call (w_scratch)
-    scratch = (lib.qb200_nf4_linear_scratch_size(n, m, n_out, k_in, int(is_bwd))
-               if cdt == torch.bfloat16 and not ex and scales is None else 0)
-    ws_bytes = max(ws_bytes, scratch)
-    assert w_scratch is None or (scales is None and w_scratch.dtype == torch.uint8 and w_scratch.device == dev)
-    if w_scratch is not None:
-        ws, ws_bytes = w_scratch, w_scratch.numel()
-    else:
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes > 0 else None
-    w_in_ws = ct.c_int(int(w_scratch is not None))
-    what = (("nf4_linear_bwd_dx" if is_bwd else "nf4_linear_fwd") + ("_lora" if r else "") + (f"_x{n}" if n > 1 else "")
-            + ("_scaled" if scales is not None else "") + ("_f16" if cdt == torch.float16 else "")
-            + ("_sf16" if twice else "") + ("_of16" if ex and out_dtype == torch.float16 else ""))
-    with torch.cuda.device(dev):
-        ev = _event_begin()
-        if scales is None:
-            rc = lib.qb200_nf4_linear_group_reuse(int(is_bwd), DTYPE_CODE[cdt], DTYPE_CODE[sdt], n, ct.addressof(probs), r, m, n_out,
-                                                  k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, ct.byref(w_in_ws), stream_ptr(dev))
-        else:
-            rc = lib.qb200_nf4_linear_group_typed(int(is_bwd), DTYPE_CODE[cdt], n, ct.addressof(probs), ct.addressof(scales), r, m,
-                                                  n_out, k_in, DTYPE_CODE[out_dtype], ptr(ws), ws_bytes, stream_ptr(dev))
-        check(rc, what)
-        _event_end(what, m * n, n_out, k_in, ev)
-    if w_in_ws.value and w_scratch is None:
-        LAUNCH_COUNTER[0] += n   # the dequantize launches that wrote the scratch
-    res = outs[0] if is_bwd else outs
+        m, f_out = inputs[0].shape[0], (k_in if is_bwd else n_out)
+        outs = [torch.empty((m, f_out), dtype=out_dtype, device=dev) for _ in range(1 if is_bwd else n)]
+    scratch = _ops.nf4_linear_group(
+        is_bwd, list(inputs), list(packeds), [a_f32 if a_u8 is None else a_u8 for a_u8, _, _, _, a_f32 in sts],
+        [t[1] for t in sts], [t[2] for t in sts], [t[3] for t in sts], n_out, k_in, states[0].dtype,
+        [] if biases is None else list(biases), [] if us is None else list(us), [] if vs is None else list(vs),
+        list(outs), out_dtype,
+        [] if row_scales is None else list(row_scales), w_scratch, return_scratch_op)
+    res = outs[0] if is_bwd else list(outs)
     if return_scratch:
-        return res, (ws if w_in_ws.value else None)
+        if not return_scratch_op or scratch.numel() == 0:
+            return res, None
+        return res, (scratch if w_scratch is None else w_scratch)
     return res
 
 
@@ -713,26 +593,10 @@ def lora_project(x2d: Tensor, lora_a: Tensor, scale: float) -> Tensor:
     bf16 (or fp16: `qb200_lora_project_typed`) operands of one dtype, fp32 sum, one rounding — what
     `torch.addmm(..., alpha=scale)` returns, in one 3 us launch that chains with the skinny kernel by programmatic dependent
     launch."""
-    dev = _require_cuda(x2d, lora_a)
     m, k = x2d.shape
-    r = lora_a.shape[0]
-    assert 1 <= m <= LORA_PROJECT_MAX_TOKENS and lora_a.shape[1] == k
+    assert 1 <= m <= LORA_PROJECT_MAX_TOKENS and lora_a.shape[1] == k and k % 8 == 0
     assert x2d.dtype in (torch.bfloat16, torch.float16) and lora_a.dtype == x2d.dtype
-    if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k or x2d.data_ptr() % 16:
-        x2d = x2d.contiguous()
-    if not lora_a.is_contiguous() or lora_a.data_ptr() % 16:
-        lora_a = lora_a.contiguous()
-    u = torch.empty((m, r), dtype=x2d.dtype, device=dev)
-    LAUNCH_COUNTER[0] += 1
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        if x2d.dtype == torch.float16:
-            rc = lib.qb200_lora_project_typed(_F16_CODE, ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u), r, m, k, r,
-                                              stream_ptr(dev))
-        else:
-            rc = lib.qb200_lora_project(ptr(x2d), x2d.stride(0), ptr(lora_a), float(scale), ptr(u), r, m, k, r, stream_ptr(dev))
-        check(rc, "lora_project")
-    return u
+    return _ops.lora_project(x2d, lora_a if lora_a.is_contiguous() else lora_a.contiguous(), float(scale))
 
 
 def nf4_linear_bwd_dx_lora(dy2d: Tensor, packed: Tensor, quant_state: QuantState, u: Tensor, vt: Tensor,
@@ -752,13 +616,17 @@ def weight_row_norm2(packed: Tensor, quant_state: QuantState) -> Tensor:
     cached = getattr(quant_state, "row_norm2", None)
     if cached is not None:
         return cached
-    if torch.cuda.is_current_stream_capturing():
+    compiling = torch.compiler.is_compiling()
+    if not compiling and torch.cuda.is_current_stream_capturing():
         raise RuntimeError("weight_row_norm2: compute the row norms of a frozen base before capturing a CUDA graph")
-    w = dequantize_4bit(packed.reshape(-1, 1), quant_state)     # [N, K] bf16 (the [1, n/2] view is not transposed back)
-    norm2 = torch.empty(w.shape[0], dtype=torch.float32, device=w.device)
-    for r0 in range(0, w.shape[0], 2048):                       # fp32 copies of 2048 rows at a time
-        norm2[r0:r0 + 2048] = w[r0:r0 + 2048].float().square().sum(1)
-    quant_state.row_norm2 = norm2
+    if quant_state.quant_type != "nf4":
+        raise NotImplementedError(f"4-bit quantization data type {quant_state.quant_type} is not implemented.")
+    n_out, k_in = quant_state.shape
+    packed = packed if packed.is_contiguous() else packed.contiguous()
+    norm2 = _ops.weight_row_norm2(packed, *_state_args(quant_state, _ops._device(packed))[:4], n_out, k_in, quant_state.dtype,
+                                  quant_state.blocksize, quant_state.state2.blocksize if quant_state.nested else 0)
+    if not compiling:   # a traced graph cannot store into the state: it computes the norms on every call without a cache
+        quant_state.row_norm2 = norm2
     return norm2
 
 

@@ -38,6 +38,7 @@ from __future__ import annotations
 
 import torch
 
+from . import _ops
 from . import functional as F
 
 
@@ -45,7 +46,9 @@ from . import functional as F
 # (`grad = 1 * grad + G^T . x`, cuBLAS beta = 1) and the autograd node returns None for them — one launch instead of a GEMM +
 # autograd's separate `grad += new` kernel per adapter matrix (448 tiny adds per Llama-2-7B step).  Only meaningful for a
 # training loop that keeps persistent `.grad` buffers and does its own gradient sync (harness/dp.py); off by default because
-# hooks on the adapter gradients (DistributedDataParallel's reducer) would never fire.
+# hooks on the adapter gradients (DistributedDataParallel's reducer) would never fire.  Each forward reads the switch once and
+# its backward follows that decision.  torch.compile reads it when it traces a graph; a traced backward cannot write into
+# `.grad`, so leave it off for compiled models.
 ACCUMULATE_ADAPTER_GRADS_IN_PLACE = False
 
 
@@ -57,19 +60,18 @@ def _scaled_mm(a: torch.Tensor, b: torch.Tensor, scale: float, out: torch.Tensor
 
 
 def _project(x2d: torch.Tensor, lora_a: torch.Tensor, scale: float) -> torch.Tensor:
-    """U = scale * x2d . lora_a^T.  A decode step (<= 16 tokens) takes the library's one-launch projection, which chains with
-    the skinny kernel by programmatic dependent launch; everything else is one cuBLAS GEMM."""
-    if (x2d.shape[0] <= F.LORA_PROJECT_MAX_TOKENS and x2d.shape[1] % 8 == 0 and x2d.dtype in (torch.bfloat16, torch.float16)
-            and lora_a.dtype == x2d.dtype and lora_a.is_contiguous()):
-        return F.lora_project(x2d, lora_a, scale)
-    return _scaled_mm(x2d, lora_a.t(), scale)
+    """U = scale * x2d . lora_a^T (`qlora_b200::lora_project`, which picks the library's decode-step projection or cuBLAS by
+    the token count at run time)."""
+    if lora_a.dtype != x2d.dtype:
+        return _scaled_mm(x2d, lora_a.t(), scale)
+    return _ops.lora_project(x2d, lora_a, float(scale))
 
 
 def _adapter_grad(param: torch.Tensor, a: torch.Tensor, b: torch.Tensor):
-    """a @ b as the gradient of `param`: returned, or (ACCUMULATE_ADAPTER_GRADS_IN_PLACE and a grad buffer exists) added in
-    place by the GEMM, in which case the node reports None."""
-    g = param.grad
-    if ACCUMULATE_ADAPTER_GRADS_IN_PLACE and g is not None and g.dtype == a.dtype and g.is_contiguous():
+    """a @ b as the gradient of `param`: returned, or added in place by the GEMM when `param` is given (its forward ran with
+    ACCUMULATE_ADAPTER_GRADS_IN_PLACE on; None otherwise) and has a grad buffer, in which case the node reports None."""
+    g = None if param is None else param.grad
+    if g is not None and g.dtype == a.dtype and g.is_contiguous():
         torch.addmm(g, a, b, out=g)
         return None
     return torch.mm(a, b)
@@ -172,7 +174,8 @@ class LoraMatMul4Bit(torch.autograd.Function):
         kept = F.scratch_to_save(scratch, ctx.needs_input_grad[0])   # a checkpoint recompute's W copies, for the dX launch
         ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs, *kept)
         ctx.kept_scratch = bool(kept)
-        ctx.adapters = (lora_as, lora_bs)   # the Parameter objects themselves (their .grad buffers, see _adapter_grad)
+        # the Parameter objects themselves, for their .grad buffers (see _adapter_grad)
+        ctx.adapters = (lora_as, lora_bs) if ACCUMULATE_ADAPTER_GRADS_IN_PLACE else ([None] * n, [None] * n)
         ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, x_loras[0] is not None
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if ctx.split else None
@@ -209,7 +212,7 @@ class LoraMatMul4Bit(torch.autograd.Function):
             grad_as = [_adapter_grad(pa[i], gs[i].t(), xls[i]) if need_a[i] else None for i in range(n)]
         else:   # one GEMM for all adapters' dA: [G_0 | G_1 | ..]^T . x
             ga_sink = None
-            if ACCUMULATE_ADAPTER_GRADS_IN_PLACE and all(a.grad is not None for a in pa):
+            if all(a is not None and a.grad is not None for a in pa):
                 ga_sink = _adjacent_rows([a.grad for a in pa])
             if ga_sink is not None and ga_sink.dtype == g_cat.dtype:
                 torch.addmm(ga_sink, g_cat.t(), xls[0], out=ga_sink)
@@ -264,8 +267,8 @@ def lora_linear4bit_group(x: torch.Tensor, bases, lora_as, lora_bs, scaling: flo
 
 def _accumulate_or_return(param: torch.Tensor, grad: torch.Tensor):
     """`grad` as the gradient of `param`, or added in place to its existing buffer (see ACCUMULATE_ADAPTER_GRADS_IN_PLACE)."""
-    g = param.grad
-    if ACCUMULATE_ADAPTER_GRADS_IN_PLACE and g is not None and g.dtype == grad.dtype and g.shape == grad.shape:
+    g = None if param is None else param.grad
+    if g is not None and g.dtype == grad.dtype and g.shape == grad.shape:
         g.add_(grad)
         return None
     return grad
@@ -293,7 +296,8 @@ class DoraMatMul4Bit(torch.autograd.Function):
             ps = F.nf4_linear_group(False, [x2d - xl for xl in xls], packeds, states)
             ys = [torch.addcmul(p.float(), q.float(), c).to(out_dtype) for p, q, c in zip(ps, qs_saved, cs)]
         ctx.save_for_backward(*xls, *us, *packeds, *lora_as, *lora_bs, *norms, *cs, *qs_saved)
-        ctx.params = (lora_as, lora_bs, mags)
+        ctx.params = (lora_as, lora_bs, mags) if ACCUMULATE_ADAPTER_GRADS_IN_PLACE else ([None] * n,) * 3
+        ctx.mag_dtypes = [m.dtype for m in mags]
         ctx.n, ctx.states, ctx.scaling, ctx.split = n, states, scaling, split
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if split else None
@@ -332,10 +336,10 @@ class DoraMatMul4Bit(torch.autograd.Function):
             grad_as = [_accumulate_or_return(pa[i], ga_cat[i * r:(i + 1) * r]) for i in range(n)]
         grad_bs, grad_ms = [], []
         for i in range(n):
-            grad_bs.append(_accumulate_or_return(pb[i], (torch.mm(g2ds[i].t(), us[i]).float() * cs[i][:, None]).to(pb[i].dtype)))
+            grad_bs.append(_accumulate_or_return(pb[i], (torch.mm(g2ds[i].t(), us[i]).float() * cs[i][:, None]).to(lora_bs[i].dtype)))
             dq = (grad_ys[i].reshape(-1, grad_ys[i].shape[-1]).float() * qs_saved[i].float()).sum(0)
             dm = dq / (norms[i] * cs[i]) if not split else dq / norms[i]
-            grad_ms.append(_accumulate_or_return(pm[i], dm.to(pm[i].dtype)))
+            grad_ms.append(_accumulate_or_return(pm[i], dm.to(ctx.mag_dtypes[i])))
         return (grad_x, None, None, None, *grad_xls, *([None] * n), *grad_as, *grad_bs, *grad_ms)
 
 
