@@ -229,6 +229,35 @@ int qb200_lora_project(const void* x, int64_t ld_x, const void* A, float scale, 
 int qb200_lora_project_typed(int dtype, const void* x, int64_t ld_x, const void* A, float scale, void* U, int64_t ld_u, int64_t M,
                              int64_t K, int64_t R, void* stream);
 
+/* ---- mixed-adapter batches: every token row uses its own LoRA adapter (peft `adapter_names`, "__base__" = none) ----------
+ * An adapter table is a DEVICE array of n_adapters entries; row_adapter a DEVICE int32 array of one adapter index per token.
+ * Token t with a(t) = row_adapter[t] in [0, n_adapters) computes, with U_t = scale_a . x_t . A_a^T rounded once to the operand
+ * type,  y_t = x_t . W^T (+bias) + U_t . B_a^T  (one rounding);  any other index means "no adapter": y_t = x_t . W^T (+bias),
+ * so no device index can make a kernel read outside the table.  A and B are dense, 16-byte aligned; rank a multiple of 8 in
+ * [8, 256] and at most the R columns of U (a kernel clamps it to those columns).  Switching a CUDA graph between batches is
+ * a copy into row_adapter: no host argument depends on which adapters the batch uses. */
+typedef struct qb200_lora_adapter {
+  const void* A;   /* lora_A.weight [rank, K] */
+  const void* B;   /* lora_B.weight [N, rank] */
+  float scale;     /* LoRA scaling */
+  int32_t rank;
+} qb200_lora_adapter;
+
+/* U[M, R] (row pitch ld_u, 0 = R) for any M >= 1: U[t, j] = scale_a . x_t . A_a[j]^T for j < rank_a, 0 for the other columns
+ * and for rows without an adapter.  Per token the arithmetic of qb200_lora_project_typed (same chunking, fp32 sum order and
+ * rounding), so a batch with one adapter gives its bits.  dtype: QB200_DTYPE_BF16 or QB200_DTYPE_F16 (x, A and U).
+ * ld_x: 0 = K.  x 16-byte and the table 8-byte aligned, K % 8 == 0; R a multiple of 8 in [8, 256] (QB200_EUNSUPPORTED
+ * otherwise). */
+int qb200_lora_project_mixed(int dtype, const void* x, int64_t ld_x, const qb200_lora_adapter* table, int n_adapters,
+                             const int32_t* row_adapter, void* U, int64_t ld_u, int64_t M, int64_t K, int64_t R, void* stream);
+
+/* qb200_nf4_linear_group_ex's forward with one adapter per token: for every problem p, probs[p].V is that linear's DEVICE
+ * adapter table (n_adapters entries, the same indices for every problem) and probs[p].U its [M, R] qb200_lora_project_mixed
+ * output; row_adapter is shared.  One skinny launch per problem (16 tokens per launch).  Token counts above
+ * QB200_SKINNY_MAX_M and an fp32 output return QB200_EUNSUPPORTED; no workspace is needed. */
+int qb200_nf4_linear_group_mixed(int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int n_adapters,
+                                 const int32_t* row_adapter, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* stream);
+
 /* ---- paged 32-bit AdamW (SURVEY.md 8f-3; qlora.py:198 optim='paged_adamw_32bit') ---------------------------
  * Replaces cadam32bit_grad_{fp32,fp16,bf16} (kernel kOptimizer32bit2State<T,ADAM>) and cget_managed_ptr / cprefetch.
  * One fused elementwise pass: p, g of `dtype`; m, v fp32; `step` counts from 1; gnorm_scale multiplies the gradient.

@@ -56,6 +56,8 @@ _SIGS = {
     "qb200_nf4_linear_group_ex": ([_i32, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, _vp], _i32),
     "qb200_nf4_linear_group_reuse": ([_i32, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp, _i64, ct.POINTER(_i32), _vp],
                                      _i32),
+    "qb200_lora_project_mixed": ([_i32, _vp, _i64, _vp, _i32, _vp, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
+    "qb200_nf4_linear_group_mixed": ([_i32, _i32, _i32, _vp, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp], _i32),
 }
 
 
@@ -65,6 +67,12 @@ class Nf4Problem(ct.Structure):
     _fields_ = [("inp", _vp), ("ld_in", _i64), ("packed", _vp), ("absmax_u8", _vp), ("code256", _vp), ("absmax2", _vp),
                 ("offset", _vp), ("absmax_f32", _vp), ("bias", _vp), ("U", _vp), ("ld_u", _i64), ("V", _vp), ("out", _vp),
                 ("ld_out", _i64)]
+
+
+class LoraAdapter(ct.Structure):
+    """`qb200_lora_adapter` of include/qlora_b200.h (one entry of a mixed-adapter table)."""
+
+    _fields_ = [("A", _vp), ("B", _vp), ("scale", ct.c_float), ("rank", ct.c_int32)]
 
 
 # upstream-named aliases (bound here only so the export test can see them)

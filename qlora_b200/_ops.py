@@ -275,6 +275,110 @@ def _(x2d, lora_a, scale):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# mixed-adapter batches: one LoRA adapter per token row, read from a device table
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _check_mixed_rows(x2d: Tensor, table: Tensor, rows: Tensor, n_adapters: int, r: int) -> None:
+    _device(x2d, table, rows)
+    assert x2d.dim() == 2 and x2d.dtype in (torch.bfloat16, torch.float16), "x2d: bf16 or fp16 [M, K]"
+    assert table.dtype == torch.uint8 and table.is_contiguous() and table.numel() == n_adapters * ct.sizeof(_lib.LoraAdapter), \
+        "table: the contiguous bytes of n_adapters qb200_lora_adapter entries"
+    assert rows.dtype == torch.int32 and rows.shape == (x2d.shape[0],) and rows.is_contiguous(), "rows: contiguous int32 [M]"
+    assert 8 <= r <= F.LORA_MAX_RANK and r % 8 == 0, "R: a multiple of 8 in [8, 256]"
+
+
+@torch.library.custom_op("qlora_b200::lora_project_mixed", mutates_args=())
+def lora_project_mixed(x2d: Tensor, table: Tensor, rows: Tensor, n_adapters: int, r: int) -> Tensor:
+    """U[M, r]: row t is scale_a . x2d[t] . A_a^T of its adapter a = rows[t] (`qb200_lora_project_mixed`), zero beyond that
+    adapter's rank and for rows without an adapter (an index outside [0, n_adapters))."""
+    _check_mixed_rows(x2d, table, rows, n_adapters, r)
+    dev = x2d.device
+    m, k = x2d.shape
+    u = torch.empty((m, r), dtype=x2d.dtype, device=dev)
+    if m == 0:
+        return u
+    if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k or x2d.data_ptr() % 16:
+        x2d = x2d.contiguous()
+    F.LAUNCH_COUNTER[0] += 1
+    with torch.cuda.device(dev):
+        check(_lib.load().qb200_lora_project_mixed(DTYPE_CODE[x2d.dtype], ptr(x2d), x2d.stride(0), ptr(table), n_adapters, ptr(rows),
+                                                   ptr(u), r, m, k, r, stream_ptr(dev)), "lora_project_mixed")
+    return u
+
+
+@lora_project_mixed.register_fake
+def _(x2d, table, rows, n_adapters, r):
+    _check_mixed_rows(x2d, table, rows, n_adapters, r)
+    return x2d.new_empty((x2d.shape[0], r))
+
+
+def _check_group_mixed(x2d, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, us, tables, rows,
+                       n_adapters, outs):
+    n = len(packeds)
+    assert len(tables) == n and len(us) == n, "one adapter table and one U per problem"
+    for t in tables:
+        _check_mixed_rows(x2d, t, rows, n_adapters, us[0].shape[1])
+    _check_group(False, [x2d] * n, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, [], [], outs,
+                 outs[0].dtype if outs else x2d.dtype, [], None)
+    r = us[0].shape[1]
+    for u in us:
+        assert u.shape == (x2d.shape[0], r) and u.dtype == x2d.dtype, f"U: {x2d.dtype} [M, {r}]"
+    assert outs[0].dtype in (torch.bfloat16, torch.float16), "out: 16-bit"
+
+
+@torch.library.custom_op("qlora_b200::nf4_linear_group_mixed", mutates_args=("outs",))
+def nf4_linear_group_mixed(x2d: Tensor, packeds: list[Tensor], absmax: list[Tensor], code2: list[Optional[Tensor]],
+                           absmax2: list[Optional[Tensor]], offset: list[Optional[Tensor]], n_out: int, k_in: int,
+                           state_dtype: torch.dtype, biases: list[Optional[Tensor]], us: list[Tensor], tables: list[Tensor],
+                           rows: Tensor, n_adapters: int, outs: list[Tensor]) -> None:
+    """out_p = x2d . W_p^T (+bias_p) + U_p[t] . B_{p,a(t)}^T for 1..3 problems of one shape on one input, a decode step
+    (`qb200_nf4_linear_group_mixed`): tables[p] is problem p's adapter table, U_p its `lora_project_mixed` output."""
+    _check_group_mixed(x2d, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, us, tables, rows,
+                       n_adapters, outs)
+    n = len(packeds)
+    m = x2d.shape[0]
+    if m == 0:
+        return
+    dev = x2d.device
+    keep = []
+    if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k_in or x2d.data_ptr() % 16:
+        x2d = x2d.contiguous()
+    probs = (_lib.Nf4Problem * n)()
+    for i in range(n):
+        packed = packeds[i] if packeds[i].is_contiguous() else packeds[i].contiguous()
+        u = us[i] if us[i].is_contiguous() else us[i].contiguous()
+        keep += [packed, u]
+        pr = probs[i]
+        pr.inp, pr.ld_in, pr.packed = x2d.data_ptr(), x2d.stride(0), packed.data_ptr()
+        if code2[i] is not None:
+            pr.absmax_u8, pr.code256, pr.absmax2, pr.offset = (absmax[i].data_ptr(), code2[i].data_ptr(), absmax2[i].data_ptr(),
+                                                               offset[i].data_ptr())
+        else:
+            pr.absmax_f32 = absmax[i].data_ptr()
+        b = biases[i] if biases else None
+        if b is not None:
+            b = b.to(x2d.dtype).contiguous()
+            keep.append(b)
+            pr.bias = b.data_ptr()
+        pr.U, pr.ld_u, pr.V = u.data_ptr(), u.stride(0), tables[i].data_ptr()
+        pr.out, pr.ld_out = outs[i].data_ptr(), outs[i].stride(0)
+    what = "nf4_linear_fwd_mixed" + (f"_x{n}" if n > 1 else "") + ("_f16" if x2d.dtype == torch.float16 else "")
+    with torch.cuda.device(dev):
+        ev = F._event_begin()
+        rc = _lib.load().qb200_nf4_linear_group_mixed(DTYPE_CODE[x2d.dtype], DTYPE_CODE[state_dtype], n, ct.addressof(probs),
+                                                      n_adapters, ptr(rows), us[0].shape[1], m, n_out, k_in,
+                                                      DTYPE_CODE[outs[0].dtype], stream_ptr(dev))
+        check(rc, what)
+        F._event_end(what, m * n, n_out, k_in, ev)
+
+
+@nf4_linear_group_mixed.register_fake
+def _(x2d, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, us, tables, rows, n_adapters, outs):
+    _check_group_mixed(x2d, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, biases, us, tables, rows,
+                       n_adapters, outs)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # NF4 and 8-bit blockwise (de)quantization
 # ----------------------------------------------------------------------------------------------------------------------
 

@@ -705,6 +705,36 @@ extern "C" int qb200_nf4_linear_group_reuse(int is_bwd, int dtype, int state_dty
                       false, w_in_workspace);
 }
 
+extern "C" int qb200_nf4_linear_group_mixed(int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int n_adapters,
+                                            const int32_t* row_adapter, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype,
+                                            void* stream) {
+  Nf4Variant v;
+  if (!nf4_variant(dtype, state_dtype, out_dtype, v))
+    return set_error(QB200_EINVAL, "nf4_linear_group_mixed: unsupported (dtype, state_dtype, out_dtype), as for nf4_linear_group_ex");
+  if (v.out_f32) return set_error(QB200_EUNSUPPORTED, "nf4_linear_group_mixed: 16-bit outputs only");
+  if (!probs || nprob < 1 || nprob > gemm::kMaxProb) return set_error(QB200_EINVAL, "nf4_linear_group: 1..3 problems per launch");
+  if (!row_adapter || n_adapters < 1) return set_error(QB200_EINVAL, "nf4_linear_group_mixed: null row_adapter or no adapters");
+  if (reinterpret_cast<uintptr_t>(row_adapter) % 4) return set_error(QB200_EINVAL, "nf4_linear_group_mixed: row_adapter must be 4-byte aligned");
+  int rc = gemm::validate_shape(M, N, K);
+  if (rc) return rc;
+  if (M > gemm::skinny_max_m()) return set_error(QB200_EUNSUPPORTED, "nf4_linear_group_mixed: skinny token counts only (QB200_SKINNY_MAX_M)");
+  if (R < 8 || R > kMaxLoraRank || R % 8 != 0)
+    return set_error(QB200_EUNSUPPORTED, "nf4_linear_group_mixed: R must be a multiple of 8 in [8, 256]");
+  const bool nested = probs[0].absmax_u8 != nullptr;
+  for (int i = 0; i < nprob; ++i) {
+    rc = gemm::validate_problem(probs[i], 0, R, N, K, true);
+    if (rc) return rc;
+    if ((probs[i].absmax_u8 != nullptr) != nested)
+      return set_error(QB200_EUNSUPPORTED, "nf4_linear_group: all problems must be nested or all plain");
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int i = 0; i < nprob; ++i) {
+    rc = launch_nf4_skinny_mixed(probs[i], row_adapter, n_adapters, int(M), int(N), int(K), int(R), v.kernels, s);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 extern "C" int64_t qb200_nf4_linear_scratch_size(int nprob, int64_t M, int64_t N, int64_t K, int is_bwd) {
   (void)is_bwd;   // the copy is W [N, K] in both directions
   if (nprob < 1 || nprob > gemm::kMaxProb || M <= 0 || N <= 0 || K <= 0 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX) return 0;

@@ -153,13 +153,14 @@ __device__ __forceinline__ SkinnyOut<T16, kOutF16> round_out(float v) {
 // B operand.  Each thread keeps kRing blocks (32 B of nibbles + absmax statistics each) in flight in registers
 // (the first version waited on one block at a time: ncu long-scoreboard 5.6 stalls / issue).
 // kStateF16: bf16 compute over an fp16 quant state (build_table); kOutF16: see SkinnyOut.
-template <typename T16, int NT, int kWarps, int kRing, bool kNested, bool kStateF16, bool kOutF16>
-__global__ void __launch_bounds__(32 * kWarps, 4)
-nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
-                  const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
-                  const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y, int M,
-                  int N, int K, const T16* __restrict__ lora_u, int ld_u, const T16* __restrict__ lora_v,
-                  int lora_r, int64_t ld_x, int64_t ld_y, const float* __restrict__ row_scale) {
+// kMixed: every token m reads its own adapter (MixedLora below): lora_v is unused and lora_r is the column count of U.
+template <typename T16, int NT, int kWarps, int kRing, bool kNested, bool kStateF16, bool kOutF16, bool kMixed>
+__device__ __forceinline__ void
+skinny_body(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+            const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
+            const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y, int M,
+            int N, int K, const T16* __restrict__ lora_u, int ld_u, const T16* __restrict__ lora_v,
+            int lora_r, int64_t ld_x, int64_t ld_y, const float* __restrict__ row_scale, MixedLora mix) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   // [kWarps][NT * 8 tokens][512 B] x slabs, then 256 floats codebook; the slabs are re-used for the partial sums at the end
   uint8_t* slab_base = smem_raw;
@@ -283,10 +284,40 @@ nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed,
     float v = 0.0f;
 #pragma unroll
     for (int w = 0; w < kWarps; ++w) v += s_red[(w * NT + nt) * 8 * kRows + i];
-    if (lora_r > 0) v += lora_dot(lora_u + int64_t(m) * ld_u, lora_v + int64_t(row) * lora_r, lora_r);
+    if constexpr (kMixed) {
+      const qb200_lora_adapter* ad = mix.adapter(m);
+      const int r = ad != nullptr ? mix.rank(*ad, lora_r) : 0;
+      if (r > 0) v += lora_dot(lora_u + int64_t(m) * ld_u, static_cast<const T16*>(ad->B) + int64_t(row) * r, r);
+    } else {
+      if (lora_r > 0) v += lora_dot(lora_u + int64_t(m) * ld_u, lora_v + int64_t(row) * lora_r, lora_r);
+    }
     if (bias != nullptr) v += widen(bias[row]);
     y[int64_t(m) * ld_y + row] = round_out<T16, kOutF16>(v);
   }
+}
+
+template <typename T16, int NT, int kWarps, int kRing, bool kNested, bool kStateF16, bool kOutF16>
+__global__ void __launch_bounds__(32 * kWarps, 4)
+nf4_skinny_kernel(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+                  const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
+                  const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y, int M,
+                  int N, int K, const T16* __restrict__ lora_u, int ld_u, const T16* __restrict__ lora_v,
+                  int lora_r, int64_t ld_x, int64_t ld_y, const float* __restrict__ row_scale) {
+  skinny_body<T16, NT, kWarps, kRing, kNested, kStateF16, kOutF16, false>(x, packed, absmax_u8, code256, absmax2, offset_ptr,
+                                                                        absmax_f32, bias, y, M, N, K, lora_u, ld_u, lora_v, lora_r,
+                                                                        ld_x, ld_y, row_scale, MixedLora{});
+}
+
+template <typename T16, int NT, int kWarps, int kRing, bool kNested, bool kStateF16, bool kOutF16>
+__global__ void __launch_bounds__(32 * kWarps, 4)
+nf4_skinny_kernel_mixed(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+                        const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
+                        const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y,
+                        int M, int N, int K, const T16* __restrict__ lora_u, int ld_u, int lora_r, int64_t ld_x, int64_t ld_y,
+                        MixedLora mix) {
+  skinny_body<T16, NT, kWarps, kRing, kNested, kStateF16, kOutF16, true>(x, packed, absmax_u8, code256, absmax2, offset_ptr,
+                                                                       absmax_f32, bias, y, M, N, K, lora_u, ld_u, nullptr, lora_r,
+                                                                       ld_x, ld_y, nullptr, mix);
 }
 
 // q's row pitches are resolved (non-zero).  Both instantiations take the full set of state pointers: the nested one reads
@@ -319,13 +350,14 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 // look-up costs 2.1 PRMT + 1.3 other ALU instructions per weight at 64 lanes/clk/SM (ncu, 4096x11008: ALU pipe 64 % of its
 // peak while SMs are active, issue slots 44 %, SMs active 71 % of the kernel) — a ceiling of ~2.7 TB/s of packed weights,
 // 0.42 of the HBM roofline, before launch and tail; DESIGN.md 4.3.
-template <typename T16, int kWarps, int kRing, int kBuf, bool kNested, bool kStateF16, bool kOutF16>
-__global__ void __launch_bounds__(32 * kWarps, 4)
-nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
-                       const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
-                       const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y,
-                       int N, int K, const T16* __restrict__ lora_u, const T16* __restrict__ lora_v, int lora_r,
-                       const float* __restrict__ row_scale) {
+// kMixed: as in skinny_body.
+template <typename T16, int kWarps, int kRing, int kBuf, bool kNested, bool kStateF16, bool kOutF16, bool kMixed>
+__device__ __forceinline__ void
+skinny_1tok_body(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+                 const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
+                 const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y,
+                 int N, int K, const T16* __restrict__ lora_u, const T16* __restrict__ lora_v, int lora_r,
+                 const float* __restrict__ row_scale, MixedLora mix) {
   using T2 = typename Vec2<T16>::type;
   constexpr int kWarpSlab = kBuf * kSlabRowBytes;
   static_assert(kRing % kBuf == 0, "the slab of ring slot u is buffer u % kBuf");
@@ -437,6 +469,11 @@ nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ pa
     s_red[warp * kRows + 2 * t] = acc[0][0] + acc[1][2];
     s_red[warp * kRows + 2 * t + 1] = acc[0][1] + acc[1][3];
   }
+  if constexpr (kMixed) {                                     // the token's own adapter, or none
+    const qb200_lora_adapter* ad = mix.adapter(0);
+    lora_r = ad != nullptr ? mix.rank(*ad, lora_r) : 0;
+    if (ad != nullptr) lora_v = static_cast<const T16*>(ad->B);
+  }
   if (lora_r > 0) {
     // 16 lanes per weight row, 4 rank entries of each 64-rank chunk each (r <= 256: up to 4 chunks), every chunk summed by
     // xor-shuffles and the chunk sums added in rank order (r <= 64: one chunk, the sum it always was).  All loads are issued
@@ -482,6 +519,42 @@ nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ pa
   }
 }
 
+template <typename T16, int kWarps, int kRing, int kBuf, bool kNested, bool kStateF16, bool kOutF16>
+__global__ void __launch_bounds__(32 * kWarps, 4)
+nf4_skinny_kernel_1tok(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+                       const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
+                       const float* __restrict__ absmax_f32, const T16* __restrict__ bias, SkinnyOut<T16, kOutF16>* __restrict__ y,
+                       int N, int K, const T16* __restrict__ lora_u, const T16* __restrict__ lora_v, int lora_r,
+                       const float* __restrict__ row_scale) {
+  skinny_1tok_body<T16, kWarps, kRing, kBuf, kNested, kStateF16, kOutF16, false>(x, packed, absmax_u8, code256, absmax2, offset_ptr,
+                                                                               absmax_f32, bias, y, N, K, lora_u, lora_v, lora_r,
+                                                                               row_scale, MixedLora{});
+}
+
+template <typename T16, int kWarps, int kRing, int kBuf, bool kNested, bool kStateF16, bool kOutF16>
+__global__ void __launch_bounds__(32 * kWarps, 4)
+nf4_skinny_kernel_1tok_mixed(const T16* __restrict__ x, const uint8_t* __restrict__ packed, const uint8_t* __restrict__ absmax_u8,
+                             const float* __restrict__ code256, const float* __restrict__ absmax2, const float* __restrict__ offset_ptr,
+                             const float* __restrict__ absmax_f32, const T16* __restrict__ bias,
+                             SkinnyOut<T16, kOutF16>* __restrict__ y, int N, int K, const T16* __restrict__ lora_u, int lora_r,
+                             MixedLora mix) {
+  skinny_1tok_body<T16, kWarps, kRing, kBuf, kNested, kStateF16, kOutF16, true>(x, packed, absmax_u8, code256, absmax2, offset_ptr,
+                                                                              absmax_f32, bias, y, N, K, lora_u, nullptr, lora_r,
+                                                                              nullptr, mix);
+}
+
+// launch_cfg with one adapter per token (nf4_skinny_kernel_mixed); q.V is unused.
+template <typename T16, bool kStateF16, bool kOutF16, int NT, int kWarps, int kRing>
+static int launch_cfg_mixed(const qb200_nf4_problem& q, const MixedLora& mix, int M, int N, int K, int R, cudaStream_t stream) {
+  constexpr int smem = kWarps * NT * 8 * kSlabRowBytes + 256 * int(sizeof(float));
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_mixed<T16, NT, kWarps, kRing, true, kStateF16, kOutF16>
+                                           : nf4_skinny_kernel_mixed<T16, NT, kWarps, kRing, false, kStateF16, kOutF16>;
+  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny_mixed", static_cast<const T16*>(q.in),
+                    q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias),
+                    static_cast<SkinnyOut<T16, kOutF16>*>(q.out), M, N, K, static_cast<const T16*>(q.U), int(q.ld_u), R, q.ld_in,
+                    q.ld_out, mix);
+}
+
 // One token: row pitches do not matter.  State pointers as in launch_cfg.
 template <typename T16, bool kStateF16, bool kOutF16, int kWarps, int kRing, int kBuf>
 static int launch_1tok(const qb200_nf4_problem& q, const float* row_scale, int N, int K, int R, cudaStream_t stream) {
@@ -496,14 +569,36 @@ static int launch_1tok(const qb200_nf4_problem& q, const float* row_scale, int N
                     row_scale);
 }
 
+// launch_1tok with the token's own adapter (nf4_skinny_kernel_1tok_mixed); q.V is unused.
+template <typename T16, bool kStateF16, bool kOutF16, int kWarps, int kRing, int kBuf>
+static int launch_1tok_mixed(const qb200_nf4_problem& q, const MixedLora& mix, int N, int K, int R, cudaStream_t stream) {
+  constexpr int kSlabs = kWarps * kBuf * kSlabRowBytes;
+  constexpr int kRed = (kWarps + 1) * kRows * int(sizeof(float));
+  constexpr int smem = (kSlabs > kRed ? kSlabs : kRed) + 256 * int(sizeof(float));
+  const auto kern = q.absmax_u8 != nullptr ? nf4_skinny_kernel_1tok_mixed<T16, kWarps, kRing, kBuf, true, kStateF16, kOutF16>
+                                           : nf4_skinny_kernel_1tok_mixed<T16, kWarps, kRing, kBuf, false, kStateF16, kOutF16>;
+  return launch_pdl(kern, unsigned(N / kRows), 32 * kWarps, smem, stream, "nf4_skinny_1tok_mixed", static_cast<const T16*>(q.in),
+                    q.packed, q.absmax_u8, q.code256, q.absmax2, q.offset, q.absmax_f32, static_cast<const T16*>(q.bias),
+                    static_cast<SkinnyOut<T16, kOutF16>*>(q.out), N, K, static_cast<const T16*>(q.U), R, mix);
+}
+
 // 16 tokens per launch (more tokens = more passes over the packed weights, which stay in L2); q's row pitches are resolved.
+// mix.table != nullptr: one adapter per token (the mixed kernels, no row scale).
 template <typename T16, bool kStateF16, bool kOutF16>
-static int launch_chunks(qb200_nf4_problem q, const float* row_scale, int M, int N, int K, int R, cudaStream_t stream) {
+static int launch_chunks(qb200_nf4_problem q, const float* row_scale, MixedLora mix, int M, int N, int K, int R, cudaStream_t stream) {
   constexpr int kChunk = 8 * kMaxNT;
   for (int m0 = 0; m0 < M; m0 += kChunk) {
     const int mc = M - m0 < kChunk ? M - m0 : kChunk;
     int rc;
-    if (mc == 1)
+    if (mix.table != nullptr) {
+      if (mc == 1)
+        rc = launch_1tok_mixed<T16, kStateF16, kOutF16, 4, 4, 2>(q, mix, N, K, R, stream);
+      else if (mc <= 8)
+        rc = launch_cfg_mixed<T16, kStateF16, kOutF16, 1, 4, 4>(q, mix, mc, N, K, R, stream);
+      else
+        rc = launch_cfg_mixed<T16, kStateF16, kOutF16, 2, 4, 4>(q, mix, mc, N, K, R, stream);
+      mix.rows += kChunk;
+    } else if (mc == 1)
       rc = launch_1tok<T16, kStateF16, kOutF16, 4, 4, 2>(q, row_scale, N, K, R, stream);
     else if (mc <= 8)
       rc = launch_cfg<T16, kStateF16, kOutF16, 1, 4, 4>(q, row_scale, mc, N, K, R, stream);
@@ -533,7 +628,22 @@ int launch_nf4_skinny(const qb200_nf4_problem& prob, const float* row_scale, int
   if (q.ld_out == 0) q.ld_out = N;
   return with_nf4_types(kernels, [&](auto t) {
     using Ty = decltype(t);
-    return skinny::launch_chunks<typename Ty::T16, Ty::kStateF16, Ty::kOutF16>(q, row_scale, M, N, K, R, stream);
+    return skinny::launch_chunks<typename Ty::T16, Ty::kStateF16, Ty::kOutF16>(q, row_scale, MixedLora{}, M, N, K, R, stream);
+  });
+}
+
+int launch_nf4_skinny_mixed(const qb200_nf4_problem& prob, const int32_t* row_adapter, int n_adapters, int M, int N, int K, int R,
+                            Nf4Kernels kernels, cudaStream_t stream) {
+  if (M < 1) return set_error(QB200_EINVAL, "nf4_skinny: M must be positive");
+  const MixedLora mix{row_adapter, static_cast<const qb200_lora_adapter*>(prob.V), n_adapters};
+  qb200_nf4_problem q = prob;
+  q.V = nullptr;
+  if (q.ld_u == 0) q.ld_u = R;
+  if (q.ld_in == 0) q.ld_in = K;
+  if (q.ld_out == 0) q.ld_out = N;
+  return with_nf4_types(kernels, [&](auto t) {
+    using Ty = decltype(t);
+    return skinny::launch_chunks<typename Ty::T16, Ty::kStateF16, Ty::kOutF16>(q, nullptr, mix, M, N, K, R, stream);
   });
 }
 

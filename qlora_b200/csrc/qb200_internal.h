@@ -85,11 +85,30 @@ auto with_nf4_types(Nf4Kernels k, Fn&& fn) {
 // per 64 ranks, the skinny kernels in 64-rank chunks of their epilogue.
 constexpr int kMaxLoraRank = 256;
 
+// The adapters of a mixed-adapter launch (qb200_lora_project_mixed, qb200_nf4_linear_group_mixed): token m uses table[rows[m]]
+// when that index is in [0, n), no adapter otherwise, so no device index can make a kernel read outside the table.
+struct MixedLora {
+  const int32_t* rows;                 // DEVICE: one adapter index per token
+  const qb200_lora_adapter* table;     // DEVICE: n entries
+  int n;
+  __device__ __forceinline__ const qb200_lora_adapter* adapter(int m) const {
+    const int a = rows[m];
+    return (a >= 0 && a < n) ? table + a : nullptr;
+  }
+  // the rank a kernel uses: the entry's, clamped to the `cols` columns of U and down to a multiple of 8 (16-byte rows)
+  __device__ __forceinline__ static int rank(const qb200_lora_adapter& ad, int cols) { return max(0, min(ad.rank, cols)) & ~7; }
+};
+
 // Forward skinny GEMM (nf4_gemv.cu) used by qb200_nf4_linear_group for M <= 16 and a 16-bit output: problem q with its
 // optional LoRA term U[M,R] . V[N,R]^T (R = 0: none) and an optional per-row weight scale row_scale[N] (null: none), run by
 // the skinny kernels of `kernels`.
 int launch_nf4_skinny(const qb200_nf4_problem& q, const float* row_scale, int M, int N, int K, int R, Nf4Kernels kernels,
                       cudaStream_t stream);
+
+// launch_nf4_skinny with one adapter per token: q.V is the DEVICE adapter table (n_adapters entries), q.U the [M, R] projection
+// of qb200_lora_project_mixed, row_adapter the DEVICE index of every token; no row scale.
+int launch_nf4_skinny_mixed(const qb200_nf4_problem& q, const int32_t* row_adapter, int n_adapters, int M, int N, int K, int R,
+                            Nf4Kernels kernels, cudaStream_t stream);
 
 // dequantize_4bit(W, state) of problem q as bf16 [N, K] into `out` (32-byte aligned) with the table kernel of nf4_quant.cu —
 // the weights the fused GEMM builds in shared memory, bit for bit (blocks of 64, nested blocks of 256).  Launched with

@@ -1,0 +1,231 @@
+"""Mixed-adapter batches over the NF4 base: each token row uses its own LoRA adapter (peft's `adapter_names`).
+
+peft's `_mixed_batch_forward` computes the base forward once, then for every adapter in the batch gathers its rows, runs
+`lora_B(lora_A(x_rows)) * scaling` and adds the result back: five small launches per adapter and linear.  Here, for row t
+with adapter a(t) (none for "__base__"):
+
+    y_t = x_t . W^T (+ bias) + [a(t) present] . U_t . B_a^T,      U_t = s_a . x_t . A_a^T  (rounded once to the compute dtype)
+
+with the sum rounded once, as `lora_linear4bit` does.
+
+* Decode (at most `DECODE_MAX_TOKENS` rows): one `lora_project_mixed` launch per linear writes U [M, R] (each row its own
+  adapter's A and scale from a device table, zero beyond its rank and for base rows), then one skinny launch per linear whose
+  epilogue reads row n of each token's own B.  No host branch depends on which adapters the batch uses, so a captured CUDA
+  graph switches requests by a copy into the row-index buffer (`LoraAdapterSet.indices(names, out=buffer)`).
+* Prefill, when the ranks of the adapters present add up to at most 256: their B matrices side by side are one V [N, sum r],
+  U [M, sum r] keeps in each row only its own adapter's block, and one existing fused (or scratch) LoRA launch runs.
+* Prefill otherwise: the rows are grouped by adapter and each group runs `lora_linear4bit`; base rows run the plain base.
+
+Inference only, as in peft: a call in grad mode with an input or adapter weight that requires grad raises.  Dropout is the
+identity.  The compute dtype is the base's (bf16, or fp16 for `compute_dtype=torch.float16`) over the quant states the fused
+path covers; the adapters are of it.
+"""
+from __future__ import annotations
+
+from typing import Sequence, Union
+
+import torch
+from torch import Tensor
+
+from . import _lib, _ops
+from . import functional as F
+from .lora import lora_linear4bit
+
+BASE_NAME = "__base__"
+DECODE_MAX_TOKENS = F.LORA_PROJECT_MAX_TOKENS
+
+
+class LoraAdapterSet:
+    """The adapters of one linear, `{name: (lora_A.weight [r, K], lora_B.weight [N, r], scaling)}`, built once.
+
+    Owns the device table the kernels read (one `qb200_lora_adapter` per adapter: pointers to A and B, scale, rank) and keeps
+    references to the weights, so no call copies them.  The table holds the weights' addresses: rebuild the set after
+    replacing a weight's storage.  Ranks are multiples of 8 in [8, 256] and may differ between adapters."""
+
+    def __init__(self, adapters: dict):
+        if not adapters:
+            raise ValueError("LoraAdapterSet: no adapters")
+        if BASE_NAME in adapters:
+            raise ValueError(f"LoraAdapterSet: {BASE_NAME!r} names the base rows, not an adapter")
+        self.names = list(adapters)
+        self.index = {name: i for i, name in enumerate(self.names)}
+        self.lora_as, self.lora_bs, self.scales, self.ranks = [], [], [], []
+        a0 = next(iter(adapters.values()))[0]
+        self.dtype, self.device = a0.dtype, a0.device
+        self.in_features = a0.shape[1]
+        self.out_features = next(iter(adapters.values()))[1].shape[0]
+        if self.dtype not in (torch.bfloat16, torch.float16) or not a0.is_cuda:
+            raise ValueError("LoraAdapterSet: bf16 or fp16 adapters on a CUDA device")
+        entries = (_lib.LoraAdapter * len(self.names))()
+        for i, (name, (a, b, scaling)) in enumerate(adapters.items()):
+            r = a.shape[0]
+            if a.dim() != 2 or b.dim() != 2 or a.shape[1] != self.in_features or b.shape != (self.out_features, r):
+                raise ValueError(f"adapter {name!r}: lora_A [r, {self.in_features}] and lora_B [{self.out_features}, r]")
+            if not (8 <= r <= F.LORA_MAX_RANK and r % 8 == 0):
+                raise ValueError(f"adapter {name!r}: rank {r} is not a multiple of 8 in [8, {F.LORA_MAX_RANK}]")
+            for t in (a, b):
+                if t.dtype != self.dtype or t.device != self.device or not t.is_contiguous() or t.data_ptr() % 16:
+                    raise ValueError(f"adapter {name!r}: contiguous, 16-byte aligned {self.dtype} weights on {self.device}")
+            self.lora_as.append(a)
+            self.lora_bs.append(b)
+            self.scales.append(float(scaling))
+            self.ranks.append(r)
+            entries[i] = _lib.LoraAdapter(a.data_ptr(), b.data_ptr(), float(scaling), r)
+        self.rmax = max(self.ranks)
+        self.table = torch.frombuffer(bytearray(bytes(entries)), dtype=torch.uint8).to(self.device)
+
+    def __len__(self) -> int:
+        return len(self.names)
+
+    def indices(self, adapter_names: Sequence[str], out: Tensor | None = None) -> Tensor:
+        """The int32 row-index tensor of `adapter_names` (-1 for "__base__") on the adapters' device, or copied into `out` (a
+        CUDA graph's index buffer).  An unknown name raises ValueError, as in peft."""
+        unknown = sorted({n for n in adapter_names if n != BASE_NAME and n not in self.index})
+        if unknown:
+            raise ValueError(f"Trying to infer with non-existing adapter(s): {', '.join(unknown)}")
+        idx = torch.tensor([self.index.get(n, -1) for n in adapter_names], dtype=torch.int32)
+        if out is None:
+            return idx.to(self.device)
+        return out.copy_(idx, non_blocking=False)
+
+    def requires_grad(self) -> bool:
+        return any(t.requires_grad for t in self.lora_as + self.lora_bs)
+
+
+def _compute_dtype(base) -> torch.dtype:
+    return torch.float16 if getattr(base, "compute_dtype", None) == torch.float16 else torch.bfloat16
+
+
+def _validate(x: Tensor, bases, sets) -> torch.dtype:
+    if not (1 <= len(bases) <= 3 and len(sets) == len(bases)):
+        raise ValueError("1..3 Linear4bit bases with one LoraAdapterSet each")
+    if torch.is_grad_enabled() and (x.requires_grad or any(s.requires_grad() for s in sets)):
+        raise RuntimeError("mixed-adapter batches are inference only (peft refuses adapter_names in training mode): call under "
+                           "torch.no_grad() or torch.inference_mode()")
+    cdt = _compute_dtype(bases[0])
+    shape = tuple(bases[0].weight.quant_state.shape)
+    for base, s in zip(bases, sets):
+        qs = base.weight.quant_state
+        if _compute_dtype(base) != cdt or tuple(qs.shape) != shape or not F.fused_supported(qs, cdt):
+            raise ValueError("mixed-adapter batches: bases of one shape and compute dtype whose quant states the fused "
+                             "kernels cover")
+        if s.dtype != cdt or (s.out_features, s.in_features) != shape:
+            raise ValueError(f"adapter set: {cdt} adapters of the base's shape")
+        if s.names != sets[0].names:
+            raise ValueError("grouped adapter sets must hold the same adapter names in the same order")
+    states = [b.weight.quant_state for b in bases]
+    if len({qs.nested for qs in states}) != 1 or len({F.double_rounded(qs, cdt) for qs in states}) != 1:
+        raise ValueError("grouped bases must share their quantization form and quant-state rounding")
+    if not (x.is_cuda and x.dtype in (cdt, torch.float32) + ((torch.float16,) if cdt == torch.bfloat16 else ())):
+        raise ValueError(f"x: a CUDA tensor of {cdt} or float32")
+    return cdt
+
+
+def _bias(base, cdt):
+    return None if base.bias is None else base.bias.to(cdt)
+
+
+def _decode(x2d: Tensor, bases, sets, rows: Tensor, cdt):
+    r = max(s.rmax for s in sets)
+    us = [_ops.lora_project_mixed(x2d, s.table, rows, len(s), r) for s in sets]
+    states = [b.weight.quant_state for b in bases]
+    sts = [F._state_tensors(qs, x2d.device) for qs in states]
+    n_out, k_in = states[0].shape
+    outs = [torch.empty((x2d.shape[0], n_out), dtype=cdt, device=x2d.device) for _ in bases]
+    _ops.nf4_linear_group_mixed(x2d, [b.weight.t() for b in bases], [a_f32 if a_u8 is None else a_u8 for a_u8, _, _, _, a_f32 in sts],
+                                [t[1] for t in sts], [t[2] for t in sts], [t[3] for t in sts], n_out, k_in, states[0].dtype,
+                                [_bias(b, cdt) for b in bases], us, [s.table for s in sets], rows, len(sets[0]), outs)
+    return outs
+
+
+def _concat_u(x2d: Tensor, s: LoraAdapterSet, present, rows: Tensor) -> Tensor:
+    """U [M, sum r]: row t keeps only the block of its own adapter (scaled, rounded once), zero elsewhere."""
+    if len(present) == 1:
+        a = present[0]
+        u = _ops.lora_project(x2d, s.lora_as[a], s.scales[a])   # lora_linear4bit's projection, bit for bit
+        return torch.where((rows == a)[:, None], u, torch.zeros((), dtype=u.dtype, device=u.device))
+    total = sum(s.ranks[a] for a in present)
+    u = torch.empty((x2d.shape[0], total), dtype=x2d.dtype, device=x2d.device)
+    lo = torch.full((len(s),), total, dtype=torch.int64)
+    c = 0
+    for a in present:   # one GEMM per adapter present, its scale as alpha: U is rounded once
+        torch.addmm(u[:, c:c + s.ranks[a]], x2d, s.lora_as[a].t(), beta=0.0, alpha=s.scales[a], out=u[:, c:c + s.ranks[a]])
+        lo[a] = c
+        c += s.ranks[a]
+    ranks = torch.tensor(s.ranks, dtype=torch.int64)
+    lo_d, hi_d = lo.to(x2d.device), (lo + ranks).to(x2d.device)
+    safe = rows.clamp(0, len(s) - 1).long()
+    row_lo = torch.where(rows >= 0, lo_d[safe], total)
+    row_hi = torch.where(rows >= 0, hi_d[safe], total)
+    col = torch.arange(total, device=x2d.device)
+    keep = (col[None, :] >= row_lo[:, None]) & (col[None, :] < row_hi[:, None])
+    return torch.where(keep, u, torch.zeros((), dtype=u.dtype, device=u.device))
+
+
+def _prefill(x2d: Tensor, bases, sets, rows: Tensor, cdt):
+    rows = torch.where((rows >= 0) & (rows < len(sets[0])), rows, -1)
+    present = sorted(a for a in set(rows.tolist()) if a >= 0)      # the one host sync of a prefill call
+    states = [b.weight.quant_state for b in bases]
+    packeds = [b.weight.t() for b in bases]
+    biases = [_bias(b, cdt) for b in bases]
+    if not present:
+        return F.nf4_linear_group(False, [x2d] * len(bases), packeds, states, biases=biases)
+    if all(sum(s.ranks[a] for a in present) <= F.LORA_MAX_RANK for s in sets):
+        us = [_concat_u(x2d, s, present, rows) for s in sets]
+        vs = [s.lora_bs[present[0]] if len(present) == 1 else torch.cat([s.lora_bs[a] for a in present], 1) for s in sets]
+        if len({u.shape[1] for u in us}) == 1:
+            return F.nf4_linear_group(False, [x2d] * len(bases), packeds, states, biases=biases, us=us, vs=vs)
+        return [F.nf4_linear_group(False, [x2d], [p], [qs], biases=[b], us=[u], vs=[v])[0]
+                for p, qs, b, u, v in zip(packeds, states, biases, us, vs)]
+    # fallback: the rows of each adapter through lora_linear4bit, the base rows through the plain base
+    outs = [torch.empty((x2d.shape[0], s.out_features), dtype=cdt, device=x2d.device) for s in sets]
+    for a in present:
+        idx = torch.nonzero(rows == a).squeeze(1)
+        xa = x2d.index_select(0, idx)
+        for out, base, s in zip(outs, bases, sets):
+            out.index_copy_(0, idx, lora_linear4bit(xa, base, s.lora_as[a], s.lora_bs[a], s.scales[a]).to(cdt))
+    idx = torch.nonzero(rows < 0).squeeze(1)
+    if idx.numel():
+        ys = F.nf4_linear_group(False, [x2d.index_select(0, idx)] * len(bases), packeds, states, biases=biases)
+        for out, y in zip(outs, ys):
+            out.index_copy_(0, idx, y)
+    return outs
+
+
+def prefill_branch(sets, adapter_names: Sequence[str]) -> str:
+    """Which prefill branch a batch takes: "concat" (ranks of the adapters present add up to at most 256, or no adapter
+    present) or "grouped" (the per-adapter fallback)."""
+    present = {n for n in adapter_names if n != BASE_NAME}
+    for s in sets:
+        if sum(s.ranks[s.index[n]] for n in present) > F.LORA_MAX_RANK:
+            return "grouped"
+    return "concat"
+
+
+def lora_linear4bit_group_mixed(x: Tensor, bases, adapter_sets, adapter_names: Union[Sequence[str], Tensor]):
+    """`[base_p(x) + per-row LoRA of adapter_sets[p]]` for 1..3 Linear4bit of one shape on one input (q/k/v, gate/up), each
+    row of `x` (flattened to [M, K]) with its own adapter.  `adapter_names`: one name per row ("__base__": no adapter), as
+    peft's `adapter_names`, or the int32 CUDA row-index tensor of `LoraAdapterSet.indices` (what a CUDA graph or a compiled
+    graph takes; an index outside [0, len(set)) means no adapter).  Returns a tuple of outputs of x's shape[:-1] + [N]."""
+    cdt = _validate(x, bases, adapter_sets)
+    x2d = F.as_compute_2d(x, cdt)
+    m = x2d.shape[0]
+    if isinstance(adapter_names, Tensor):
+        rows = adapter_names
+        if rows.dtype != torch.int32 or rows.shape != (m,) or rows.device != x2d.device:
+            raise ValueError(f"row indices: int32 [{m}] on {x2d.device}")
+    else:
+        if len(adapter_names) != m:
+            raise ValueError(f"adapter_names: one name per row, {m} rows, got {len(adapter_names)}")
+        rows = adapter_sets[0].indices(adapter_names)
+    rows = rows if rows.is_contiguous() else rows.contiguous()
+    ys = _decode(x2d, bases, adapter_sets, rows, cdt) if m <= DECODE_MAX_TOKENS else _prefill(x2d, bases, adapter_sets, rows, cdt)
+    out_dtype = F.out_dtype_for(x.dtype, cdt)
+    n_out = bases[0].weight.quant_state.shape[0]
+    return tuple((y if y.dtype == out_dtype else y.to(out_dtype)).view(*x.shape[:-1], n_out) for y in ys)
+
+
+def lora_linear4bit_mixed(x: Tensor, base, adapters: LoraAdapterSet, adapter_names: Union[Sequence[str], Tensor]) -> Tensor:
+    """`base(x)` plus, for every row of x, the LoRA update of its own adapter in `adapters` (peft's mixed batch forward for
+    one Linear4bit).  See `lora_linear4bit_group_mixed`."""
+    return lora_linear4bit_group_mixed(x, [base], [adapters], adapter_names)[0]

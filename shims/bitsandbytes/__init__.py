@@ -15,6 +15,8 @@ import qlora_b200 as _impl  # noqa: E402
 from qlora_b200 import MatMul4Bit, matmul_4bit  # noqa: E402,F401
 from qlora_b200 import lora_linear4bit, lora_linear4bit_group  # noqa: E402,F401  (extensions: fused LoRA step, SURVEY.md 8f-1)
 from qlora_b200 import dora_linear4bit, dora_linear4bit_group, dora_linear4bit_peft  # noqa: E402,F401  (extensions: fused QDoRA)
+# extensions: mixed-adapter batches (peft adapter_names)
+from qlora_b200 import LoraAdapterSet, lora_linear4bit_group_mixed, lora_linear4bit_mixed  # noqa: E402,F401
 from qlora_b200 import functional, nn, optim  # noqa: E402,F401
 
 __version__ = _impl.__version__
