@@ -258,6 +258,37 @@ int qb200_lora_project_mixed(int dtype, const void* x, int64_t ld_x, const qb200
 int qb200_nf4_linear_group_mixed(int dtype, int state_dtype, int nprob, const qb200_nf4_problem* probs, int n_adapters,
                                  const int32_t* row_adapter, int64_t R, int64_t M, int64_t N, int64_t K, int out_dtype, void* stream);
 
+/* Segmented LoRA: a mixed-adapter batch of any token count with no read-back to the host.  The rows are grouped by adapter on
+ * the device (qb200_lora_segment_table), then tensor-core kernels run one tile of up to 64 rows of one adapter per CTA.
+ * For a batch of M rows over an adapter table of n_adapters entries:
+ *   1. y = the base launch (qb200_nf4_linear_group_ex without LoRA operands), 16-bit;
+ *   2. U [M, R] = qb200_lora_project_mixed, or qb200_lora_shrink_segmented (rows with an adapter only);
+ *   3. qb200_lora_segment_table;
+ *   4. qb200_lora_expand_segmented: y_t = rn(y_t + U_t . B_a^T), fp32 sum, in place; rows without an adapter keep y's bits.
+ * The result is rounded twice (the base output, then the sum), where qb200_nf4_linear_group_mixed rounds once.  Indices and
+ * ranks are clamped as in qb200_lora_project_mixed.  Argument errors return QB200_EINVAL (QB200_EUNSUPPORTED for an R outside
+ * the multiples of 8 in [8, 256]) before any launch. */
+
+/* Bytes of the segment table's workspace for M rows and n_adapters adapters; it depends on nothing else.  0 for M < 1,
+ * n_adapters < 1 or a table too large for one grid. */
+int64_t qb200_lora_segment_workspace_size(int64_t M, int n_adapters);
+/* The segment table of the DEVICE row indices row_adapter [M] into the lent DEVICE workspace (16-byte aligned, at least
+ * qb200_lora_segment_workspace_size bytes): a stable counting sort of the rows into one bucket per adapter plus one for
+ * "no adapter", the bucket offsets and the list of 64-row tiles the two kernels below run over.  One CTA. */
+int qb200_lora_segment_table(const int32_t* row_adapter, int64_t M, int n_adapters, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+/* U_p[t, j] = rn(scale_a . x_t . A_a[j]^T) for the rows t with an adapter a and j < rank_a, 0 for j in [rank_a, R); rows
+ * without an adapter are not written.  x [M, K] (ld_x: 0 = K) is shared by the nprob (1..3) problems, tables[p] and U[p] are
+ * problem p's DEVICE adapter table and [M, R] output (ld_u: 0 = R).  dtype: QB200_DTYPE_BF16 or QB200_DTYPE_F16. */
+int qb200_lora_shrink_segmented(int dtype, int nprob, const void* x, int64_t ld_x, const qb200_lora_adapter* const* tables,
+                                void* const* U, int64_t ld_u, int n_adapters, const void* workspace, int64_t workspace_bytes,
+                                int64_t M, int64_t K, int64_t R, void* stream);
+/* out_p[t] = rn(out_p[t] + U_p[t] . B_a^T) over N columns (a multiple of 8; ld_out: 0 = N, even) for every row t with an
+ * adapter a, in place; U[p] [M, R] (ld_u: 0 = R, a multiple of 8, 16-byte aligned) and tables[p] as for the shrink. */
+int qb200_lora_expand_segmented(int dtype, int nprob, const qb200_lora_adapter* const* tables, const void* const* U, int64_t ld_u,
+                                void* const* out, int64_t ld_out, int n_adapters, const void* workspace, int64_t workspace_bytes,
+                                int64_t M, int64_t N, int64_t R, void* stream);
+
 /* ---- paged 32-bit AdamW (SURVEY.md 8f-3; qlora.py:198 optim='paged_adamw_32bit') ---------------------------
  * Replaces cadam32bit_grad_{fp32,fp16,bf16} (kernel kOptimizer32bit2State<T,ADAM>) and cget_managed_ptr / cprefetch.
  * One fused elementwise pass: p, g of `dtype`; m, v fp32; `step` counts from 1; gnorm_scale multiplies the gradient.

@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libqlora_b200.so")
-SOURCES = ["qb200_api.cu", "nf4_quant.cu", "nf4_gemm_sm90.cu", "nf4_gemv.cu", "lora_proj.cu", "paged_optim.cu", "optim32.cu"]
+SOURCES = ["qb200_api.cu", "nf4_quant.cu", "nf4_gemm_sm90.cu", "nf4_gemv.cu", "lora_proj.cu", "lora_segmented.cu", "paged_optim.cu", "optim32.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -58,6 +58,10 @@ _SIGS = {
                                      _i32),
     "qb200_lora_project_mixed": ([_i32, _vp, _i64, _vp, _i32, _vp, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
     "qb200_nf4_linear_group_mixed": ([_i32, _i32, _i32, _vp, _i32, _vp, _i64, _i64, _i64, _i64, _i32, _vp], _i32),
+    "qb200_lora_segment_workspace_size": ([_i64, _i32], _i64),
+    "qb200_lora_segment_table": ([_vp, _i64, _i32, _vp, _i64, _vp], _i32),
+    "qb200_lora_shrink_segmented": ([_i32, _i32, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
+    "qb200_lora_expand_segmented": ([_i32, _i32, _vp, _vp, _i64, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
 }
 
 

@@ -378,6 +378,72 @@ def _(x2d, packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, bi
                        n_adapters, outs)
 
 
+# From this many (token rows x problems) on, U comes from the segmented tensor-core shrink, which reads each row of x once
+# per 128 ranks but runs one CTA per 64-row tile and problem over the whole contraction; below it, from
+# `qb200_lora_project_mixed`, which reads x once per rank but spreads a small batch over R x M / 8 CTAs.  On an H100 (r = 64,
+# 1 to 16 adapters) the shrink was faster from 256 rows for q/k/v (3 problems, K = 4096) and from 1024 rows for down
+# (1 problem, K = 11008), and slower at 512 rows for down.
+SEGMENTED_SHRINK_MIN_WORK = 768
+
+
+def _check_segmented(x2d: Tensor, tables: list[Tensor], rows: Tensor, n_adapters: int, r: int, outs: list[Tensor]) -> None:
+    assert 1 <= len(tables) <= 3 and len(outs) == len(tables), "1..3 problems, one adapter table and one output each"
+    for t in tables:
+        _check_mixed_rows(x2d, t, rows, n_adapters, r)
+    _device(x2d, *outs)
+    m = x2d.shape[0]
+    n_out = outs[0].shape[1] if outs else 0
+    for o in outs:
+        assert o.dim() == 2 and o.shape == (m, n_out) and o.dtype == x2d.dtype and o.is_contiguous(), \
+            f"out: contiguous {x2d.dtype} [{m}, N]"
+    assert n_out % 8 == 0, "N: a multiple of 8"
+
+
+@torch.library.custom_op("qlora_b200::lora_segmented_add", mutates_args=("outs",))
+def lora_segmented_add(x2d: Tensor, tables: list[Tensor], rows: Tensor, n_adapters: int, r: int, outs: list[Tensor]) -> None:
+    """outs[p][t] = rn(outs[p][t] + U_p[t] . B_{p,a}^T) for every row t whose index a = rows[t] is in [0, n_adapters), with
+    U_p[t] = rn(s_a . x2d[t] . A_{p,a}^T) of tables[p]; the other rows are not written.  Any token count, no host sync: the
+    segment table (`qb200_lora_segment_table`), U (`qb200_lora_project_mixed` per problem when rows x
+    problems is below SEGMENTED_SHRINK_MIN_WORK, else one `qb200_lora_shrink_segmented`) and one `qb200_lora_expand_segmented`
+    for all problems.  The choice is made here at run time, so a graph traced with a symbolic token count serves both."""
+    _check_segmented(x2d, tables, rows, n_adapters, r, outs)
+    m, k = x2d.shape
+    if m == 0:
+        return
+    dev = x2d.device
+    n = len(tables)
+    if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k or x2d.data_ptr() % 16:
+        x2d = x2d.contiguous()
+    lib = _lib.load()
+    ws_bytes = lib.qb200_lora_segment_workspace_size(m, n_adapters)
+    assert ws_bytes > 0, "lora_segmented_add: too many rows and adapters for one segment table"
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    us = [torch.empty((m, r), dtype=x2d.dtype, device=dev) for _ in range(n)]
+    table_ptrs = (ct.c_void_p * n)(*[t.data_ptr() for t in tables])
+    u_ptrs = (ct.c_void_p * n)(*[u.data_ptr() for u in us])
+    out_ptrs = (ct.c_void_p * n)(*[o.data_ptr() for o in outs])
+    dt = DTYPE_CODE[x2d.dtype]
+    shrink = m * n >= SEGMENTED_SHRINK_MIN_WORK
+    F.LAUNCH_COUNTER[0] += 2 + (1 if shrink else n)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(lib.qb200_lora_segment_table(ptr(rows), m, n_adapters, ptr(ws), ws_bytes, s), "lora_segment_table")
+        if shrink:
+            check(lib.qb200_lora_shrink_segmented(dt, n, ptr(x2d), x2d.stride(0), table_ptrs, u_ptrs, r, n_adapters, ptr(ws), ws_bytes,
+                                                  m, k, r, s), "lora_shrink_segmented")
+        else:
+            for t, u in zip(tables, us):
+                check(lib.qb200_lora_project_mixed(dt, ptr(x2d), x2d.stride(0), ptr(t), n_adapters, ptr(rows), ptr(u), r, m, k, r, s),
+                      "lora_project_mixed")
+        check(lib.qb200_lora_expand_segmented(dt, n, table_ptrs, u_ptrs, r, out_ptrs, outs[0].stride(0), n_adapters, ptr(ws),
+                                              ws_bytes, m, outs[0].shape[1], r, s), "lora_expand_segmented")
+
+
+@lora_segmented_add.register_fake
+def _(x2d, tables, rows, n_adapters, r, outs):
+    _check_segmented(x2d, tables, rows, n_adapters, r, outs)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # NF4 and 8-bit blockwise (de)quantization
 # ----------------------------------------------------------------------------------------------------------------------

@@ -6,15 +6,24 @@ with adapter a(t) (none for "__base__"):
 
     y_t = x_t . W^T (+ bias) + [a(t) present] . U_t . B_a^T,      U_t = s_a . x_t . A_a^T  (rounded once to the compute dtype)
 
-with the sum rounded once, as `lora_linear4bit` does.
+with the sum rounded once, as `lora_linear4bit` does, except on the segmented path below.
 
 * Decode (at most `DECODE_MAX_TOKENS` rows): one `lora_project_mixed` launch per linear writes U [M, R] (each row its own
   adapter's A and scale from a device table, zero beyond its rank and for base rows), then one skinny launch per linear whose
   epilogue reads row n of each token's own B.  No host branch depends on which adapters the batch uses, so a captured CUDA
   graph switches requests by a copy into the row-index buffer (`LoraAdapterSet.indices(names, out=buffer)`).
-* Prefill, when the ranks of the adapters present add up to at most 256: their B matrices side by side are one V [N, sum r],
-  U [M, sum r] keeps in each row only its own adapter's block, and one existing fused (or scratch) LoRA launch runs.
-* Prefill otherwise: the rows are grouped by adapter and each group runs `lora_linear4bit`; base rows run the plain base.
+* Above `DECODE_MAX_TOKENS` rows, the row-index tensor form takes the segmented path at every token count: the base launch
+  without LoRA operands, then `lora_segmented_add`, which groups the rows by adapter on the device and adds each row's own
+  U . B_a^T in place with tensor-core kernels.  No host branch depends on the indices and nothing is read back to the host,
+  so such a batch too can be captured in a CUDA graph or compiled.  It rounds twice: the base output (`Linear4bit`'s bits,
+  which rows without an adapter keep), then the sum.
+* The names form above `DECODE_MAX_TOKENS` rows picks its branch from the names on the host (`prefill_branch`).  When the
+  ranks of the adapters present add up to at most 256 ("concat"): their B matrices side by side are one V [N, sum r],
+  U [M, sum r] keeps in each row only its own adapter's block, and one existing fused (or scratch) LoRA launch runs, with
+  one rounding.  Otherwise ("grouped"): the adapters present are split into groups of at most 256 ranks, and the rows of
+  each group run that concat launch on their own, so each NF4 weight is read once per group; one rounding too.  The names
+  form keeps one rounding because, under bf16 compute, the segmented path's two roundings exceed the Frobenius-relative
+  1e-3 bar against float64 that `lora_linear4bit` meets (2.3e-3 measured at 1600 rows); every element stays within 1 ulp.
 
 Inference only, as in peft: a call in grad mode with an input or adapter weight that requires grad raises.  Dropout is the
 identity.  The compute dtype is the base's (bf16, or fp16 for `compute_dtype=torch.float16`) over the quant states the fused
@@ -29,7 +38,6 @@ from torch import Tensor
 
 from . import _lib, _ops
 from . import functional as F
-from .lora import lora_linear4bit
 
 BASE_NAME = "__base__"
 DECODE_MAX_TOKENS = F.LORA_PROJECT_MAX_TOKENS
@@ -162,39 +170,65 @@ def _concat_u(x2d: Tensor, s: LoraAdapterSet, present, rows: Tensor) -> Tensor:
     return torch.where(keep, u, torch.zeros((), dtype=u.dtype, device=u.device))
 
 
-def _prefill(x2d: Tensor, bases, sets, rows: Tensor, cdt):
-    rows = torch.where((rows >= 0) & (rows < len(sets[0])), rows, -1)
-    present = sorted(a for a in set(rows.tolist()) if a >= 0)      # the one host sync of a prefill call
-    states = [b.weight.quant_state for b in bases]
-    packeds = [b.weight.t() for b in bases]
-    biases = [_bias(b, cdt) for b in bases]
-    if not present:
-        return F.nf4_linear_group(False, [x2d] * len(bases), packeds, states, biases=biases)
-    if all(sum(s.ranks[a] for a in present) <= F.LORA_MAX_RANK for s in sets):
-        us = [_concat_u(x2d, s, present, rows) for s in sets]
-        vs = [s.lora_bs[present[0]] if len(present) == 1 else torch.cat([s.lora_bs[a] for a in present], 1) for s in sets]
-        if len({u.shape[1] for u in us}) == 1:
-            return F.nf4_linear_group(False, [x2d] * len(bases), packeds, states, biases=biases, us=us, vs=vs)
-        return [F.nf4_linear_group(False, [x2d], [p], [qs], biases=[b], us=[u], vs=[v])[0]
-                for p, qs, b, u, v in zip(packeds, states, biases, us, vs)]
-    # fallback: the rows of each adapter through lora_linear4bit, the base rows through the plain base
-    outs = [torch.empty((x2d.shape[0], s.out_features), dtype=cdt, device=x2d.device) for s in sets]
+def _base_outs(x2d: Tensor, bases, cdt):
+    return F.nf4_linear_group(False, [x2d] * len(bases), [b.weight.t() for b in bases], [b.weight.quant_state for b in bases],
+                              biases=[_bias(b, cdt) for b in bases])
+
+
+def _segmented(x2d: Tensor, bases, sets, rows: Tensor, cdt):
+    outs = _base_outs(x2d, bases, cdt)
+    _ops.lora_segmented_add(x2d, [s.table for s in sets], rows, len(sets[0]), max(s.rmax for s in sets), outs)
+    return outs
+
+
+def _rank_groups(sets, present):
+    """The adapters present split, in index order, into groups whose ranks add up to at most 256 in every set."""
+    groups, cur = [], []
     for a in present:
-        idx = torch.nonzero(rows == a).squeeze(1)
-        xa = x2d.index_select(0, idx)
-        for out, base, s in zip(outs, bases, sets):
-            out.index_copy_(0, idx, lora_linear4bit(xa, base, s.lora_as[a], s.lora_bs[a], s.scales[a]).to(cdt))
-    idx = torch.nonzero(rows < 0).squeeze(1)
-    if idx.numel():
-        ys = F.nf4_linear_group(False, [x2d.index_select(0, idx)] * len(bases), packeds, states, biases=biases)
+        if cur and any(sum(s.ranks[b] for b in cur) + s.ranks[a] > F.LORA_MAX_RANK for s in sets):
+            groups.append(cur)
+            cur = []
+        cur.append(a)
+    return groups + [cur]
+
+
+def _grouped(x2d: Tensor, bases, sets, rows: Tensor, names, cdt):
+    """Σr > 256: the adapters present in groups of at most 256 ranks; the rows of each group (known on the host from the
+    names) through one concat launch, the base rows through the plain base.  One rounding per row, as the concat branch;
+    each NF4 weight is read once per group rather than once per adapter."""
+    index = sets[0].index
+    by_adapter = {}
+    for t, name in enumerate(names):
+        by_adapter.setdefault(index.get(name, -1), []).append(t)
+    outs = [torch.empty((x2d.shape[0], s.out_features), dtype=cdt, device=x2d.device) for s in sets]
+    present = sorted(a for a in by_adapter if a >= 0)
+    for group in _rank_groups(sets, present) + ([None] if -1 in by_adapter else []):
+        ts = by_adapter[-1] if group is None else sorted(t for a in group for t in by_adapter[a])
+        idx = torch.tensor(ts, dtype=torch.long).to(x2d.device)
+        xg = x2d.index_select(0, idx)
+        ys = _base_outs(xg, bases, cdt) if group is None else _concat(xg, bases, sets, rows.index_select(0, idx), group, cdt)
         for out, y in zip(outs, ys):
             out.index_copy_(0, idx, y)
     return outs
 
 
+def _concat(x2d: Tensor, bases, sets, rows: Tensor, present, cdt):
+    if not present:
+        return _base_outs(x2d, bases, cdt)
+    states = [b.weight.quant_state for b in bases]
+    packeds = [b.weight.t() for b in bases]
+    biases = [_bias(b, cdt) for b in bases]
+    us = [_concat_u(x2d, s, present, rows) for s in sets]
+    vs = [s.lora_bs[present[0]] if len(present) == 1 else torch.cat([s.lora_bs[a] for a in present], 1) for s in sets]
+    if len({u.shape[1] for u in us}) == 1:
+        return F.nf4_linear_group(False, [x2d] * len(bases), packeds, states, biases=biases, us=us, vs=vs)
+    return [F.nf4_linear_group(False, [x2d], [p], [qs], biases=[b], us=[u], vs=[v])[0]
+            for p, qs, b, u, v in zip(packeds, states, biases, us, vs)]
+
+
 def prefill_branch(sets, adapter_names: Sequence[str]) -> str:
-    """Which prefill branch a batch takes: "concat" (ranks of the adapters present add up to at most 256, or no adapter
-    present) or "grouped" (the per-adapter fallback)."""
+    """Which branch a batch of names takes above `DECODE_MAX_TOKENS` rows: "concat" (ranks of the adapters present add up to
+    at most 256, or no adapter present) or "grouped" (the rows grouped by adapter, one concat launch per 256 ranks)."""
     present = {n for n in adapter_names if n != BASE_NAME}
     for s in sets:
         if sum(s.ranks[s.index[n]] for n in present) > F.LORA_MAX_RANK:
@@ -219,7 +253,15 @@ def lora_linear4bit_group_mixed(x: Tensor, bases, adapter_sets, adapter_names: U
             raise ValueError(f"adapter_names: one name per row, {m} rows, got {len(adapter_names)}")
         rows = adapter_sets[0].indices(adapter_names)
     rows = rows if rows.is_contiguous() else rows.contiguous()
-    ys = _decode(x2d, bases, adapter_sets, rows, cdt) if m <= DECODE_MAX_TOKENS else _prefill(x2d, bases, adapter_sets, rows, cdt)
+    if m <= DECODE_MAX_TOKENS:
+        ys = _decode(x2d, bases, adapter_sets, rows, cdt)
+    elif isinstance(adapter_names, Tensor):
+        ys = _segmented(x2d, bases, adapter_sets, rows, cdt)
+    elif prefill_branch(adapter_sets, adapter_names) == "concat":
+        present = sorted({adapter_sets[0].index[n] for n in adapter_names if n != BASE_NAME})
+        ys = _concat(x2d, bases, adapter_sets, rows, present, cdt)
+    else:
+        ys = _grouped(x2d, bases, adapter_sets, rows, adapter_names, cdt)
     out_dtype = F.out_dtype_for(x.dtype, cdt)
     n_out = bases[0].weight.quant_state.shape[0]
     return tuple((y if y.dtype == out_dtype else y.to(out_dtype)).view(*x.shape[:-1], n_out) for y in ys)
