@@ -52,7 +52,7 @@ constexpr int kSmemTiles = kStages * (kInSlotBytes + kATileBytes);   // 192 KB
 constexpr int kSmemBytes = kSmemTiles + kAuxBytes + 1024;
 
 struct Maps {
-  CUtensorMap in[kMaxProb];   // activations In_p[T, C]   (forward groups: the same tensor for every problem)
+  CUtensorMap in[kMaxProb];   // activations In_p[T, C]: each problem's own input and row pitch
   CUtensorMap u[kMaxProb];    // LoRA U_p[T, r]
   CUtensorMap v[kMaxProb];    // LoRA V_p: [F, r] forward, [r, F] dX
 };
