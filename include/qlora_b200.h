@@ -289,6 +289,41 @@ int qb200_lora_expand_segmented(int dtype, int nprob, const qb200_lora_adapter* 
                                 void* const* out, int64_t ld_out, int n_adapters, const void* workspace, int64_t workspace_bytes,
                                 int64_t M, int64_t N, int64_t R, void* stream);
 
+/* Segmented LoRA backward: training several adapters over one base in one batch.  For the forward above (U_p saved), dY_p
+ * the output gradients and the same segment table:
+ *   G_p [M, R]   = qb200_lora_grad_shrink_segmented     G_p[t] = rn(s_a . dY_p[t] . B_a), zero beyond rank_a;
+ *   dX           = the base dX launch (16-bit), then qb200_lora_grad_input_segmented with accumulate = 1:
+ *                  dX[t] = rn(dX[t] + sum_p G_p[t] . A_{p,a}), the problems summed in fp32 before the one rounding;
+ *                  or, when each problem's adapter reads its own (dropped) input, accumulate = 0: dxl_p[t] = rn(G_p[t] . A_{p,a});
+ *   dA_p, dB_p   = qb200_lora_weight_grad_segmented     dA_a = rn(sum_{rows of a} G^T . x_lora), dB_a = rn(sum dY^T . U).
+ * Every sum is fp32 in a fixed order (no atomics), so equal inputs give equal bits.  Rows without an adapter are not written
+ * by the first two; indices and ranks are clamped as in qb200_lora_project_mixed.  Argument errors return QB200_EINVAL
+ * (QB200_EUNSUPPORTED for an R outside the multiples of 8 in [8, 256]) before any launch. */
+
+/* G[p][t, j] = rn(scale_a . dY[p][t] . B_a[:, j]) for j < rank_a, 0 for j in [rank_a, R), over the N columns of dY[p]
+ * (N a multiple of 8; ld_dy: 0 = N, a multiple of 8, 16-byte aligned rows); G[p] [M, R] (ld_g: 0 = R, even).  tables[p] as for
+ * qb200_lora_shrink_segmented. */
+int qb200_lora_grad_shrink_segmented(int dtype, int nprob, const void* const* dY, int64_t ld_dy, const qb200_lora_adapter* const* tables,
+                                     void* const* G, int64_t ld_g, int n_adapters, const void* workspace, int64_t workspace_bytes,
+                                     int64_t M, int64_t N, int64_t R, void* stream);
+/* accumulate = 1: dx[0][t] = rn(dx[0][t] + sum_p G[p][t] . A_{p,a}) in place (dx[0] only is read);  accumulate = 0:
+ * dx[p][t] = rn(G[p][t] . A_{p,a}).  K columns (a multiple of 8; ld_dx: 0 = K, even), G[p] [M, R] (ld_g: 0 = R, a multiple
+ * of 8, 16-byte aligned). */
+int qb200_lora_grad_input_segmented(int dtype, int nprob, int accumulate, const qb200_lora_adapter* const* tables,
+                                    const void* const* G, int64_t ld_g, void* const* dx, int64_t ld_dx, int n_adapters,
+                                    const void* workspace, int64_t workspace_bytes, int64_t M, int64_t K, int64_t R, void* stream);
+/* For each adapter a and problem p, over the rows t of a (the segment table's bucket, in sorted order):
+ *   D_a[i, j] = rn(sum_t P[p][t, i] . Q[p][t, j]),  i < rank_a, j < D,
+ * written to out[p] at element rank_offsets[a] . D: transpose_out = 0 as [rank_a, D] (dA_a: P = G, Q = the adapters' input,
+ * D = K), 1 as [D, rank_a] (dB_a: P = U, Q = dY, D = N).  rank_offsets is a DEVICE int64 [n_adapters] array (8-byte aligned)
+ * of the ranks' exclusive prefix sums, shared by the problems; each out[p] holds rank_total . D elements, and an adapter
+ * whose offset would write past them writes nothing.  An adapter without rows gets zeros.  P[p] [M, R] (ld_p: 0 = R) and
+ * Q[p] [M, D] (ld_q: 0 = D), 16-byte aligned; D a multiple of 8. */
+int qb200_lora_weight_grad_segmented(int dtype, int nprob, int transpose_out, const qb200_lora_adapter* const* tables,
+                                     const int64_t* rank_offsets, int64_t rank_total, const void* const* P, int64_t ld_p,
+                                     const void* const* Q, int64_t ld_q, void* const* out, int n_adapters, const void* workspace,
+                                     int64_t workspace_bytes, int64_t M, int64_t D, int64_t R, void* stream);
+
 /* ---- paged 32-bit AdamW (SURVEY.md 8f-3; qlora.py:198 optim='paged_adamw_32bit') ---------------------------
  * Replaces cadam32bit_grad_{fp32,fp16,bf16} (kernel kOptimizer32bit2State<T,ADAM>) and cget_managed_ptr / cprefetch.
  * One fused elementwise pass: p, g of `dtype`; m, v fp32; `step` counts from 1; gnorm_scale multiplies the gradient.

@@ -62,6 +62,10 @@ _SIGS = {
     "qb200_lora_segment_table": ([_vp, _i64, _i32, _vp, _i64, _vp], _i32),
     "qb200_lora_shrink_segmented": ([_i32, _i32, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
     "qb200_lora_expand_segmented": ([_i32, _i32, _vp, _vp, _i64, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
+    "qb200_lora_grad_shrink_segmented": ([_i32, _i32, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
+    "qb200_lora_grad_input_segmented": ([_i32, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
+    "qb200_lora_weight_grad_segmented": ([_i32, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _vp, _i64, _i64, _i64, _i64,
+                                          _vp], _i32),
 }
 
 

@@ -407,41 +407,183 @@ def lora_segmented_add(x2d: Tensor, tables: list[Tensor], rows: Tensor, n_adapte
     problems is below SEGMENTED_SHRINK_MIN_WORK, else one `qb200_lora_shrink_segmented`) and one `qb200_lora_expand_segmented`
     for all problems.  The choice is made here at run time, so a graph traced with a symbolic token count serves both."""
     _check_segmented(x2d, tables, rows, n_adapters, r, outs)
-    m, k = x2d.shape
+    m = x2d.shape[0]
     if m == 0:
         return
-    dev = x2d.device
-    n = len(tables)
-    if x2d.stride(1) != 1 or x2d.stride(0) % 8 or x2d.stride(0) < k or x2d.data_ptr() % 16:
-        x2d = x2d.contiguous()
-    lib = _lib.load()
-    ws_bytes = lib.qb200_lora_segment_workspace_size(m, n_adapters)
-    assert ws_bytes > 0, "lora_segmented_add: too many rows and adapters for one segment table"
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    us = [torch.empty((m, r), dtype=x2d.dtype, device=dev) for _ in range(n)]
-    table_ptrs = (ct.c_void_p * n)(*[t.data_ptr() for t in tables])
-    u_ptrs = (ct.c_void_p * n)(*[u.data_ptr() for u in us])
-    out_ptrs = (ct.c_void_p * n)(*[o.data_ptr() for o in outs])
-    dt = DTYPE_CODE[x2d.dtype]
-    shrink = m * n >= SEGMENTED_SHRINK_MIN_WORK
-    F.LAUNCH_COUNTER[0] += 2 + (1 if shrink else n)
-    with torch.cuda.device(dev):
-        s = stream_ptr(dev)
-        check(lib.qb200_lora_segment_table(ptr(rows), m, n_adapters, ptr(ws), ws_bytes, s), "lora_segment_table")
-        if shrink:
-            check(lib.qb200_lora_shrink_segmented(dt, n, ptr(x2d), x2d.stride(0), table_ptrs, u_ptrs, r, n_adapters, ptr(ws), ws_bytes,
-                                                  m, k, r, s), "lora_shrink_segmented")
-        else:
-            for t, u in zip(tables, us):
-                check(lib.qb200_lora_project_mixed(dt, ptr(x2d), x2d.stride(0), ptr(t), n_adapters, ptr(rows), ptr(u), r, m, k, r, s),
-                      "lora_project_mixed")
-        check(lib.qb200_lora_expand_segmented(dt, n, table_ptrs, u_ptrs, r, out_ptrs, outs[0].stride(0), n_adapters, ptr(ws),
-                                              ws_bytes, m, outs[0].shape[1], r, s), "lora_expand_segmented")
+    ws = torch.empty(segment_workspace_bytes(m, n_adapters), dtype=torch.uint8, device=x2d.device)
+    _segmented_add([x2d], tables, rows, n_adapters, r, outs, [torch.empty((m, r), dtype=x2d.dtype, device=x2d.device) for _ in tables],
+                   ws)
 
 
 @lora_segmented_add.register_fake
 def _(x2d, tables, rows, n_adapters, r, outs):
     _check_segmented(x2d, tables, rows, n_adapters, r, outs)
+
+
+def segment_workspace_bytes(m, n_adapters: int):
+    """`qb200_lora_segment_workspace_size(m, n_adapters)` (seg::layout in lora_segmented.cu), also for a symbolic m."""
+    pad = lambda b: (b + 15) // 16 * 16  # noqa: E731
+    return pad(4 * m) + pad(4 * (n_adapters + 2)) + 16 * ((m + 63) // 64 + n_adapters) + pad(8 * (n_adapters + 1))
+
+
+def _rows_2d(t: Tensor) -> Tensor:
+    """t as rows the segmented kernels read: unit stride, a row pitch of a multiple of 8 elements, 16-byte aligned."""
+    if t.stride(1) != 1 or t.stride(0) % 8 or t.stride(0) < t.shape[1] or t.data_ptr() % 16:
+        return t.contiguous()
+    return t
+
+
+def _segmented_add(xs, tables, rows, n_adapters, r, outs, us, ws) -> None:
+    """The segment table into `ws`, U_p into `us` and outs[p] += U_p . B^T: `lora_segmented_add` (one shared input in `xs`)
+    and `lora_segmented_fwd` (one input per problem: each problem's U from its own input, one launch per problem)."""
+    xs = [_rows_2d(x) for x in xs]
+    m, k = xs[0].shape
+    dev = xs[0].device
+    n = len(tables)
+    lib = _lib.load()
+    ws_bytes = lib.qb200_lora_segment_workspace_size(m, n_adapters)
+    assert ws_bytes > 0 and ws.numel() >= ws_bytes, "segmented LoRA: too many rows and adapters for one segment table"
+    table_ptrs = (ct.c_void_p * n)(*[t.data_ptr() for t in tables])
+    u_ptrs = (ct.c_void_p * n)(*[u.data_ptr() for u in us])
+    out_ptrs = (ct.c_void_p * n)(*[o.data_ptr() for o in outs])
+    dt = DTYPE_CODE[xs[0].dtype]
+    shrink = m * n >= SEGMENTED_SHRINK_MIN_WORK
+    F.LAUNCH_COUNTER[0] += 2 + (len(xs) if shrink else n)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(lib.qb200_lora_segment_table(ptr(rows), m, n_adapters, ptr(ws), ws_bytes, s), "lora_segment_table")
+        if shrink and len(xs) == 1:
+            x2d = xs[0]
+            check(lib.qb200_lora_shrink_segmented(dt, n, ptr(x2d), x2d.stride(0), table_ptrs, u_ptrs, r, n_adapters, ptr(ws), ws_bytes,
+                                                  m, k, r, s), "lora_shrink_segmented")
+        else:
+            for i, (t, u) in enumerate(zip(tables, us)):
+                x2d = xs[i % len(xs)]
+                if shrink:
+                    check(lib.qb200_lora_shrink_segmented(dt, 1, ptr(x2d), x2d.stride(0), (ct.c_void_p * 1)(t.data_ptr()),
+                                                          (ct.c_void_p * 1)(u.data_ptr()), r, n_adapters, ptr(ws), ws_bytes, m, k,
+                                                          r, s), "lora_shrink_segmented")
+                else:
+                    check(lib.qb200_lora_project_mixed(dt, ptr(x2d), x2d.stride(0), ptr(t), n_adapters, ptr(rows), ptr(u), r, m, k, r,
+                                                       s), "lora_project_mixed")
+        check(lib.qb200_lora_expand_segmented(dt, n, table_ptrs, u_ptrs, r, out_ptrs, outs[0].stride(0), n_adapters, ptr(ws),
+                                              ws_bytes, m, outs[0].shape[1], r, s), "lora_expand_segmented")
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# training several adapters in one batch: the segmented forward that keeps U and the segment table, and its backward
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _check_segmented_fwd(xs, tables, rows, n_adapters, r, outs) -> None:
+    assert len(xs) in (1, len(tables)), "one input shared by the problems, or one per problem"
+    for x in xs:
+        _check_segmented(x, tables, rows, n_adapters, r, outs)
+        assert x.shape == xs[0].shape, "the problems' inputs share one shape"
+
+
+@torch.library.custom_op("qlora_b200::lora_segmented_fwd", mutates_args=("outs",))
+def lora_segmented_fwd(xs: list[Tensor], tables: list[Tensor], rows: Tensor, n_adapters: int, r: int,
+                       outs: list[Tensor]) -> tuple[Tensor, Tensor]:
+    """`lora_segmented_add` that returns what the backward reads: (U [P, M, r], the segment table's workspace).  With one
+    input in `xs` it runs exactly `lora_segmented_add`'s launches; with one input per problem (the adapters' dropped inputs),
+    U_p is computed from xs[p]."""
+    _check_segmented_fwd(xs, tables, rows, n_adapters, r, outs)
+    m = xs[0].shape[0]
+    dev = xs[0].device
+    us = torch.empty((len(tables), m, r), dtype=xs[0].dtype, device=dev)
+    ws = torch.empty(segment_workspace_bytes(m, n_adapters), dtype=torch.uint8, device=dev)
+    if m:
+        _segmented_add(xs, tables, rows, n_adapters, r, outs, list(us.unbind(0)), ws)
+    return us, ws
+
+
+@lora_segmented_fwd.register_fake
+def _(xs, tables, rows, n_adapters, r, outs):
+    _check_segmented_fwd(xs, tables, rows, n_adapters, r, outs)
+    m = xs[0].shape[0]
+    return xs[0].new_empty((len(tables), m, r)), xs[0].new_empty((segment_workspace_bytes(m, n_adapters),), dtype=torch.uint8)
+
+
+def _check_segmented_bwd(g2ds, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dx, split):
+    n = len(tables)
+    assert 1 <= n <= 3 and len(g2ds) == n and len(xls) in (1, n), "1..3 problems: one dY each, one adapter input or one each"
+    _device(*g2ds, *tables, rank_offsets, us, *xls, ws, dx)
+    m, n_out = g2ds[0].shape
+    cdt = g2ds[0].dtype
+    assert cdt in (torch.bfloat16, torch.float16), "dY: bf16 or fp16"
+    for g in g2ds:
+        assert g.shape == (m, n_out) and g.dtype == cdt, f"dY: {cdt} [{m}, {n_out}]"
+    k = xls[0].shape[1]
+    for x in xls:
+        assert x.dim() == 2 and x.shape == (m, k) and x.dtype == cdt, f"adapter input: {cdt} [{m}, K]"
+    for t in tables:
+        assert t.dtype == torch.uint8 and t.is_contiguous() and t.numel() == n_adapters * ct.sizeof(_lib.LoraAdapter), \
+            "table: the contiguous bytes of n_adapters qb200_lora_adapter entries"
+    assert rank_offsets.dtype == torch.int64 and rank_offsets.shape == (n_adapters,) and rank_offsets.is_contiguous(), \
+        "rank_offsets: contiguous int64 [n_adapters]"
+    assert 8 <= r <= F.LORA_MAX_RANK and r % 8 == 0 and rank_total >= 8, "R: a multiple of 8 in [8, 256]; rank_total >= 8"
+    assert us.shape == (n, m, r) and us.dtype == cdt and us.is_contiguous(), f"U: contiguous {cdt} [{n}, {m}, {r}]"
+    assert ws.dtype == torch.uint8 and ws.dim() == 1, "ws: the forward's segment table"
+    assert n_out % 8 == 0 and k % 8 == 0, "N and K: multiples of 8"
+    assert dx is None or (not split and dx.shape == (m, k) and dx.dtype == cdt and dx.stride(1) == 1), \
+        f"dx: {cdt} [{m}, {k}] rows (no dropout input only)"
+    assert not split or len(xls) == n, "split: one adapter input per problem"
+    return m, n_out, k, cdt
+
+
+@torch.library.custom_op("qlora_b200::lora_segmented_bwd", mutates_args=("dx",))
+def lora_segmented_bwd(g2ds: list[Tensor], tables: list[Tensor], rank_offsets: Tensor, rank_total: int, us: Tensor,
+                       xls: list[Tensor], ws: Tensor, n_adapters: int, r: int, dx: Optional[Tensor],
+                       split: bool) -> tuple[Tensor, Tensor, Tensor]:
+    """The LoRA part of a segmented backward, over the forward's U and segment table `ws`:
+    G_p = rn(s_a . dY_p . B_{p,a}) (`qb200_lora_grad_shrink_segmented`); then, without dropout, dx += sum_p G_p . A_{p,a} in
+    place on the base dX launch's output (or nothing when `dx` is None), with dropout (`split`) dxl_p = rn(G_p . A_{p,a}); and
+    the flat weight gradients: dA [P, rank_total . K] (adapter a's [r_a, K] at rank_offsets[a] . K) and dB
+    [P, rank_total . N] ([N, r_a] at rank_offsets[a] . N) (`qb200_lora_weight_grad_segmented`).
+    Returns (dxl [P, M, K] with `split`, else an empty tensor; dA; dB)."""
+    m, n_out, k, cdt = _check_segmented_bwd(g2ds, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dx, split)
+    n = len(tables)
+    dev = g2ds[0].device
+    dxl = torch.zeros((n, m, k) if split else (0,), dtype=cdt, device=dev)
+    d_a = torch.empty((n, rank_total * k), dtype=cdt, device=dev)
+    d_b = torch.empty((n, rank_total * n_out), dtype=cdt, device=dev)
+    if m == 0:
+        return dxl, d_a.zero_(), d_b.zero_()
+    g2ds = [g.contiguous() for g in g2ds]
+    xls = [x.contiguous() for x in xls] * (n // len(xls))
+    gs = torch.empty((n, m, r), dtype=cdt, device=dev)
+    lib = _lib.load()
+    ws_bytes = ws.numel()
+    assert ws_bytes >= lib.qb200_lora_segment_workspace_size(m, n_adapters), "ws: the forward's segment table for these rows"
+    arr = lambda ts: (ct.c_void_p * n)(*[t.data_ptr() for t in ts])  # noqa: E731
+    tables_p, gs_p = arr(tables), arr(gs.unbind(0))
+    dt = DTYPE_CODE[cdt]
+    F.LAUNCH_COUNTER[0] += 3 + int(split or dx is not None)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(lib.qb200_lora_grad_shrink_segmented(dt, n, arr(g2ds), n_out, tables_p, gs_p, r, n_adapters, ptr(ws), ws_bytes, m, n_out,
+                                                   r, s), "lora_grad_shrink_segmented")
+        if split:
+            check(lib.qb200_lora_grad_input_segmented(dt, n, 0, tables_p, gs_p, r, arr(dxl.unbind(0)), k, n_adapters, ptr(ws),
+                                                      ws_bytes, m, k, r, s), "lora_grad_input_segmented")
+        elif dx is not None:
+            check(lib.qb200_lora_grad_input_segmented(dt, n, 1, tables_p, gs_p, r, arr([dx] * n), dx.stride(0), n_adapters, ptr(ws),
+                                                      ws_bytes, m, k, r, s), "lora_grad_input_segmented")
+        check(lib.qb200_lora_weight_grad_segmented(dt, n, 0, tables_p, ptr(rank_offsets), rank_total, gs_p, r, arr(xls), k,
+                                                   arr(d_a.unbind(0)), n_adapters, ptr(ws), ws_bytes, m, k, r, s),
+              "lora_weight_grad_segmented")
+        check(lib.qb200_lora_weight_grad_segmented(dt, n, 1, tables_p, ptr(rank_offsets), rank_total, arr(us.unbind(0)), r,
+                                                   arr(g2ds), n_out, arr(d_b.unbind(0)), n_adapters, ptr(ws), ws_bytes, m, n_out,
+                                                   r, s), "lora_weight_grad_segmented")
+    return dxl, d_a, d_b
+
+
+@lora_segmented_bwd.register_fake
+def _(g2ds, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dx, split):
+    m, n_out, k, cdt = _check_segmented_bwd(g2ds, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dx, split)
+    n = len(tables)
+    g = g2ds[0]
+    return (g.new_empty((n, m, k) if split else (0,)), g.new_empty((n, rank_total * k)), g.new_empty((n, rank_total * n_out)))
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -26,7 +26,8 @@ with the sum rounded once, as `lora_linear4bit` does, except on the segmented pa
   1e-3 bar against float64 that `lora_linear4bit` meets (2.3e-3 measured at 1600 rows); every element stays within 1 ulp.
 
 Inference only, as in peft: a call in grad mode with an input or adapter weight that requires grad raises.  Dropout is the
-identity.  The compute dtype is the base's (bf16, or fp16 for `compute_dtype=torch.float16`) over the quant states the fused
+identity.  Training takes `lora_linear4bit_group_multi` / `lora_linear4bit_multi` (end of this file): the segmented forward
+at every token count, differentiable in the input and every adapter's weights (DESIGN.md §6d).  The compute dtype is the base's (bf16, or fp16 for `compute_dtype=torch.float16`) over the quant states the fused
 path covers; the adapters are of it.
 """
 from __future__ import annotations
@@ -81,6 +82,11 @@ class LoraAdapterSet:
             entries[i] = _lib.LoraAdapter(a.data_ptr(), b.data_ptr(), float(scaling), r)
         self.rmax = max(self.ranks)
         self.table = torch.frombuffer(bytearray(bytes(entries)), dtype=torch.uint8).to(self.device)
+        # adapter a's rows in the flat weight-gradient buffers of `lora_linear4bit_group_multi`: [offsets[a], offsets[a] + r_a)
+        offsets = [sum(self.ranks[:i]) for i in range(len(self.ranks))]
+        self.rank_offsets_host = offsets
+        self.rank_total = sum(self.ranks)
+        self.rank_offsets = torch.tensor(offsets, dtype=torch.int64).to(self.device)
 
     def __len__(self) -> int:
         return len(self.names)
@@ -104,10 +110,10 @@ def _compute_dtype(base) -> torch.dtype:
     return torch.float16 if getattr(base, "compute_dtype", None) == torch.float16 else torch.bfloat16
 
 
-def _validate(x: Tensor, bases, sets) -> torch.dtype:
+def _validate(x: Tensor, bases, sets, training: bool = False) -> torch.dtype:
     if not (1 <= len(bases) <= 3 and len(sets) == len(bases)):
         raise ValueError("1..3 Linear4bit bases with one LoraAdapterSet each")
-    if torch.is_grad_enabled() and (x.requires_grad or any(s.requires_grad() for s in sets)):
+    if not training and torch.is_grad_enabled() and (x.requires_grad or any(s.requires_grad() for s in sets)):
         raise RuntimeError("mixed-adapter batches are inference only (peft refuses adapter_names in training mode): call under "
                            "torch.no_grad() or torch.inference_mode()")
     cdt = _compute_dtype(bases[0])
@@ -271,3 +277,102 @@ def lora_linear4bit_mixed(x: Tensor, base, adapters: LoraAdapterSet, adapter_nam
     """`base(x)` plus, for every row of x, the LoRA update of its own adapter in `adapters` (peft's mixed batch forward for
     one Linear4bit).  See `lora_linear4bit_group_mixed`."""
     return lora_linear4bit_group_mixed(x, [base], [adapters], adapter_names)[0]
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# training several adapters over one base in one batch (DESIGN.md §6d)
+# ----------------------------------------------------------------------------------------------------------------------
+
+class MultiLoraMatMul4Bit(torch.autograd.Function):
+    """y_p[t] = x[t] . W_p^T (+bias_p) + U_p[t] . B_{p,a}^T with U_p[t] = rn(s_{p,a} . xl_p[t] . A_{p,a}^T), a = rows[t], for
+    n = 1..3 Linear4bit of one shape on one input; xl_p = x without dropout.  The forward is the segmented forward of
+    `lora_linear4bit_group_mixed` (`lora_segmented_fwd`, which also returns U and the segment table); the backward is
+    the base dX launch plus `lora_segmented_bwd`.  Differentiable in x, the dropped inputs and every adapter's A and B."""
+
+    @staticmethod
+    def forward(ctx, x, rows, states, sets, n: int, *tensors):
+        x_loras, packeds, biases = (list(tensors[i * n:(i + 1) * n]) for i in range(3))
+        cdt = sets[0].dtype
+        x2d = F.as_compute_2d(x, cdt)
+        split = x_loras[0] is not None
+        xls = [F.as_compute_2d(t, cdt) for t in x_loras] if split else [x2d]
+        outs = F.nf4_linear_group(False, [x2d] * n, packeds, list(states), biases=biases)
+        r = max(s.rmax for s in sets)
+        us, ws = _ops.lora_segmented_fwd(xls, [s.table for s in sets], rows, len(sets[0]), r, outs)
+        ctx.save_for_backward(us, ws, *xls, *packeds)
+        ctx.n, ctx.states, ctx.sets, ctx.r, ctx.split = n, states, sets, r, split
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if split else None
+        out_dtype = F.out_dtype_for(x.dtype, cdt)
+        n_out = states[0].shape[0]
+        return tuple((y if y.dtype == out_dtype else y.to(out_dtype)).view(*x.shape[:-1], n_out) for y in outs)
+
+    @staticmethod
+    def backward(ctx, *grad_ys):
+        n, sets, split = ctx.n, ctx.sets, ctx.split
+        us, ws, *rest = ctx.saved_tensors
+        xls, packeds = rest[:len(rest) - n], rest[len(rest) - n:]
+        need = ctx.needs_input_grad
+        need_xl = need[5:5 + n]
+        n_ad = len(sets[0])
+        cdt = sets[0].dtype
+        g2ds = [F.as_compute_2d(g, cdt) for g in grad_ys]
+        dx = F.nf4_linear_group(True, g2ds, packeds, list(ctx.states), out_dtype=cdt) if need[0] else None
+        # without dropout the adapters' input-gradient term is added in place to the base dX; with it, to each dropped input
+        dxl, d_a, d_b = _ops.lora_segmented_bwd(g2ds, [s.table for s in sets], sets[0].rank_offsets, sets[0].rank_total, us,
+                                                list(xls), ws, n_ad, ctx.r, None if split else dx, split)
+        grad_x = None if dx is None else dx.to(ctx.x_dtype).view(ctx.x_shape)
+        grad_xls = [None] * n
+        if split:
+            for p in range(n):
+                if need_xl[p]:
+                    shape, dtype = ctx.xl_meta[p]
+                    grad_xls[p] = dxl[p].to(dtype).view(shape)
+        k, n_out = xls[0].shape[1], g2ds[0].shape[1]
+        offs, ranks = sets[0].rank_offsets_host, sets[0].ranks
+        base = 5 + 3 * n
+        grad_as = [d_a[p, offs[a] * k:(offs[a] + ranks[a]) * k].view(ranks[a], k) if need[base + p * n_ad + a] else None
+                   for p in range(n) for a in range(n_ad)]
+        base += n * n_ad
+        grad_bs = [d_b[p, offs[a] * n_out:(offs[a] + ranks[a]) * n_out].view(n_out, ranks[a]) if need[base + p * n_ad + a] else None
+                   for p in range(n) for a in range(n_ad)]
+        return (grad_x, None, None, None, None, *grad_xls, *([None] * 2 * n), *grad_as, *grad_bs)
+
+
+def _rows_tensor(rows, sets, m: int, device) -> Tensor:
+    if isinstance(rows, Tensor):
+        if rows.dtype != torch.int32 or rows.shape != (m,) or rows.device != device:
+            raise ValueError(f"row indices: int32 [{m}] on {device}")
+        return rows if rows.is_contiguous() else rows.contiguous()
+    if len(rows) != m:
+        raise ValueError(f"adapter_names: one name per row, {m} rows, got {len(rows)}")
+    return sets[0].indices(rows)
+
+
+def lora_linear4bit_group_multi(x: Tensor, bases, adapter_sets, rows: Union[Sequence[str], Tensor], x_loras=None):
+    """`lora_linear4bit_group_mixed` for training: `[base_p(x) + per-row LoRA of adapter_sets[p]]` for 1..3 Linear4bit of one
+    shape on one input, differentiable in `x`, in `x_loras` and in every adapter's lora_A and lora_B held by the sets, so one
+    batch trains several adapters over one frozen base.  `rows`: the int32 row-index tensor of `LoraAdapterSet.indices`
+    (an index outside [0, len(set)) means no adapter), or one name per row.  `x_loras`: each problem's dropped input (peft's
+    `lora_dropout`), of x's shape; None: the adapters read x.  The sets hold the same names with the same ranks.
+
+    Every token count takes the segmented path, so no host branch depends on the indices and a step can be captured in a
+    CUDA graph or compiled.  The gradients of the adapters' weights are views of one flat buffer per problem and kind."""
+    cdt = _validate(x, bases, adapter_sets, training=True)
+    if any(s.ranks != adapter_sets[0].ranks for s in adapter_sets):
+        raise ValueError("grouped adapter sets must give each adapter the same rank")
+    n = len(bases)
+    if x_loras is not None:
+        if len(x_loras) != n or any(t.shape != x.shape or t.device != x.device for t in x_loras):
+            raise ValueError("x_loras: one input of x's shape per base")
+    m = x.numel() // x.shape[-1] if x.shape[-1] else 0
+    rows = _rows_tensor(rows, adapter_sets, m, x.device)
+    tensors = [*(x_loras if x_loras is not None else [None] * n), *[b.weight.t() for b in bases], *[_bias(b, cdt) for b in bases],
+               *[a for s in adapter_sets for a in s.lora_as], *[b for s in adapter_sets for b in s.lora_bs]]
+    return MultiLoraMatMul4Bit.apply(x, rows, tuple(b.weight.quant_state for b in bases), tuple(adapter_sets), n, *tensors)
+
+
+def lora_linear4bit_multi(x: Tensor, base, adapter_set: LoraAdapterSet, rows: Union[Sequence[str], Tensor],
+                          x_lora: Tensor | None = None) -> Tensor:
+    """`lora_linear4bit_group_multi` for one Linear4bit: `base(x)` plus each row's own adapter, trainable."""
+    return lora_linear4bit_group_multi(x, [base], [adapter_set], rows, None if x_lora is None else [x_lora])[0]
