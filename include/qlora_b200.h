@@ -324,6 +324,51 @@ int qb200_lora_weight_grad_segmented(int dtype, int nprob, int transpose_out, co
                                      const void* const* Q, int64_t ld_q, void* const* out, int n_adapters, const void* workspace,
                                      int64_t workspace_bytes, int64_t M, int64_t D, int64_t R, void* stream);
 
+/* Segmented DoRA (QDoRA): several DoRA adapters over one NF4 base in one batch (DESIGN.md §6e).  Adapter a of problem p has
+ * the table entry {A, B, s, r} of the LoRA kernels above and a magnitude m_a [N] of the compute dtype; with the detached norm
+ * n_a[f] = ||W_f + s . (B_a A_a)_f|| and c_a = m_a / n_a (fp32 [n_adapters, N] per problem):
+ *   norms    qb200_dora_stack_a, the fused forward P = A_stack . W^T with an fp32 output, qb200_dora_norm_segmented;
+ *   forward  the base launch (and, with dropout, Qb = rn(xd . W^T)), U as for the LoRA forward, qb200_dora_expand_segmented;
+ *   backward qb200_dora_grad_scale_segmented, then the LoRA backward's launches with dQ in place of dY.
+ * The ranks are shared by the problems: rank_offsets [n_adapters] (DEVICE int64, the ranks' exclusive prefix sums, 8-byte
+ * aligned) place adapter a's rows in [off_a, off_a + r_a) of rank_total.  An entry whose rank is not a positive multiple of 8
+ * or whose offset would reach past rank_total is unusable: its rows take the base only, as rows without an adapter do.  Every
+ * sum is fp32 in a fixed order (no atomics).  Argument errors return QB200_EINVAL (QB200_EUNSUPPORTED for an R outside the
+ * multiples of 8 in [8, 256]) before any launch.  dtype: QB200_DTYPE_BF16 or QB200_DTYPE_F16. */
+
+/* out[p] [rank_total, K] (16-byte aligned): row j = A_{p,a}[j - off_a] of the adapter a = stack_rows[j] (DEVICE int32
+ * [rank_total]), zeros for a row outside its adapter's clamped rank.  K a multiple of 8. */
+int qb200_dora_stack_a(int dtype, int nprob, const qb200_lora_adapter* const* tables, const int32_t* stack_rows,
+                       const int64_t* rank_offsets, int64_t rank_total, void* const* out, int n_adapters, int64_t K, int64_t R,
+                       void* stream);
+/* Two launches: gram[p] (fp32, gram_total elements) holds G_a = A_a . A_a^T [r_a, r_a] at gram_offsets[a] (DEVICE int64,
+ * exclusive prefix sums of r_a^2); then c[p] and norm[p] (fp32 [n_adapters, N], 8-byte aligned) get, for every row f,
+ *   n_a[f] = sqrt(max(0, row_norm2[p][f] + 2 s_a sum_j B_a[f, j] P[p][off_a + j, f] + s_a^2 (B_a G_a B_a^T)[f, f])),
+ *   c_a[f] = m_a[f] / n_a[f],
+ * with P[p] [rank_total, N] fp32 from the fused forward over qb200_dora_stack_a's rows, row_norm2[p] = ||W_f||^2 fp32 [N], and
+ * mag_tables[p] a DEVICE array of n_adapters pointers to the magnitudes.  An unusable entry gets c = n = 0. */
+int qb200_dora_norm_segmented(int dtype, int nprob, const qb200_lora_adapter* const* tables, const void* const* mag_tables,
+                              const int64_t* rank_offsets, const int64_t* gram_offsets, int64_t rank_total, int64_t gram_total,
+                              const float* const* P, const float* const* row_norm2, float* const* gram, float* const* c,
+                              float* const* norm, int n_adapters, int64_t N, int64_t K, int64_t R, void* stream);
+/* qb200_lora_expand_segmented with the magnitude scale c[p] (fp32 [n_adapters, N], 8-byte aligned) of each row's adapter,
+ * over the segment table of the forward:  dropout = 0: out_p[t] = rn(c_a . (out_p[t] + U_p[t] . B_a^T));  dropout = 1:
+ * out_p[t] = rn(out_p[t] + (c_a - 1) . Q_p[t] + c_a . U_p[t] . B_a^T) and Q_p[t] = rn(Q_p[t] + U_p[t] . B_a^T) in place, Q_p
+ * read as rn(xd_p . W_p^T) (row pitch ld_out).  Rows without an adapter are not written. */
+int qb200_dora_expand_segmented(int dtype, int nprob, int dropout, const qb200_lora_adapter* const* tables, const void* const* U,
+                                int64_t ld_u, const float* const* c, void* const* Q, void* const* out, int64_t ld_out, int n_adapters,
+                                const void* workspace, int64_t workspace_bytes, int64_t M, int64_t N, int64_t R, void* stream);
+/* Per problem p and row t of adapter a (the forward's segment table):  dQ[p][t] = rn(dY[p][t] . c_a);  dropout = 1 also
+ * dD[p][t] = rn(dY[p][t] . (c_a - 1));  dm[p][a . N + f] = rn(sum_{t of a} dY[p][t, f] . Q[p][t, f] / n_a[f]), the sum fp32
+ * in sorted-row order.  Q[p] is the expand's pre-scale output with dropout, else the forward's output y, read as y / c_a (an
+ * element with c_a = 0 adds nothing).  Rows without a usable adapter copy dY into dQ and get dD = 0; an adapter without rows
+ * gets dm = 0.  dY, Q, dQ and dD share the row pitch ld (0 = N, even); dm[p] holds n_adapters . N elements. */
+int qb200_dora_grad_scale_segmented(int dtype, int nprob, int dropout, const qb200_lora_adapter* const* tables,
+                                    const int64_t* rank_offsets, int64_t rank_total, const void* const* dY, const void* const* Q,
+                                    const float* const* c, const float* const* norm, int64_t ld, void* const* dQ, void* const* dD,
+                                    void* const* dm, int n_adapters, const void* workspace, int64_t workspace_bytes, int64_t M,
+                                    int64_t N, int64_t R, void* stream);
+
 /* ---- paged 32-bit AdamW (SURVEY.md 8f-3; qlora.py:198 optim='paged_adamw_32bit') ---------------------------
  * Replaces cadam32bit_grad_{fp32,fp16,bf16} (kernel kOptimizer32bit2State<T,ADAM>) and cget_managed_ptr / cprefetch.
  * One fused elementwise pass: p, g of `dtype`; m, v fp32; `step` counts from 1; gnorm_scale multiplies the gradient.

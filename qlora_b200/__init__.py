@@ -13,6 +13,7 @@ from .lora import LoraMatMul4Bit, lora_linear4bit, lora_linear4bit_group  # noqa
 from .lora import DoraMatMul4Bit, dora_linear4bit, dora_linear4bit_group, dora_linear4bit_peft  # noqa: F401
 from .mixed import LoraAdapterSet, lora_linear4bit_group_mixed, lora_linear4bit_mixed  # noqa: F401
 from .mixed import MultiLoraMatMul4Bit, lora_linear4bit_group_multi, lora_linear4bit_multi  # noqa: F401
+from .mixed import DoraAdapterSet, MultiDoraMatMul4Bit, dora_linear4bit_group_multi, dora_linear4bit_multi  # noqa: F401
 
 # transformers gates 4-bit support on `bitsandbytes.__version__ >= 0.46.1`
 __version__ = "0.46.1"

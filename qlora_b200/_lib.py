@@ -66,6 +66,13 @@ _SIGS = {
     "qb200_lora_grad_input_segmented": ([_i32, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp], _i32),
     "qb200_lora_weight_grad_segmented": ([_i32, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _vp, _i64, _i64, _i64, _i64,
                                           _vp], _i32),
+    "qb200_dora_stack_a": ([_i32, _i32, _vp, _vp, _vp, _i64, _vp, _i32, _i64, _i64, _vp], _i32),
+    "qb200_dora_norm_segmented": ([_i32, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _i64, _vp],
+                                  _i32),
+    "qb200_dora_expand_segmented": ([_i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _i64, _i64, _i64, _vp],
+                                    _i32),
+    "qb200_dora_grad_scale_segmented": ([_i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp, _i64,
+                                         _i64, _i64, _i64, _vp], _i32),
 }
 
 

@@ -433,9 +433,10 @@ def _rows_2d(t: Tensor) -> Tensor:
     return t
 
 
-def _segmented_add(xs, tables, rows, n_adapters, r, outs, us, ws) -> None:
+def _segmented_add(xs, tables, rows, n_adapters, r, outs, us, ws, dora=None) -> None:
     """The segment table into `ws`, U_p into `us` and outs[p] += U_p . B^T: `lora_segmented_add` (one shared input in `xs`)
-    and `lora_segmented_fwd` (one input per problem: each problem's U from its own input, one launch per problem)."""
+    and `lora_segmented_fwd` (one input per problem: each problem's U from its own input, one launch per problem).
+    `dora` = (c [P, n, N], [Q_p] or []): the expand is `qb200_dora_expand_segmented` (`dora_segmented_fwd`)."""
     xs = [_rows_2d(x) for x in xs]
     m, k = xs[0].shape
     dev = xs[0].device
@@ -466,6 +467,12 @@ def _segmented_add(xs, tables, rows, n_adapters, r, outs, us, ws) -> None:
                 else:
                     check(lib.qb200_lora_project_mixed(dt, ptr(x2d), x2d.stride(0), ptr(t), n_adapters, ptr(rows), ptr(u), r, m, k, r,
                                                        s), "lora_project_mixed")
+        if dora is not None:
+            cs, qs = dora
+            check(lib.qb200_dora_expand_segmented(dt, n, int(bool(qs)), table_ptrs, u_ptrs, r, _ptrs(cs.unbind(0)),
+                                                  _ptrs(qs) if qs else None, out_ptrs, outs[0].stride(0), n_adapters, ptr(ws),
+                                                  ws_bytes, m, outs[0].shape[1], r, s), "dora_expand_segmented")
+            return
         check(lib.qb200_lora_expand_segmented(dt, n, table_ptrs, u_ptrs, r, out_ptrs, outs[0].stride(0), n_adapters, ptr(ws),
                                               ws_bytes, m, outs[0].shape[1], r, s), "lora_expand_segmented")
 
@@ -584,6 +591,232 @@ def _(g2ds, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dx, sp
     n = len(tables)
     g = g2ds[0]
     return (g.new_empty((n, m, k) if split else (0,)), g.new_empty((n, rank_total * k)), g.new_empty((n, rank_total * n_out)))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# training several DoRA adapters in one batch (DESIGN.md §6e): the norms of every adapter, the scaled expand and the
+# gradient scale
+# ----------------------------------------------------------------------------------------------------------------------
+
+def _ptrs(ts):
+    return (ct.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+def _check_tables(tables, n_adapters):
+    for t in tables:
+        assert t.dtype == torch.uint8 and t.is_contiguous() and t.numel() == n_adapters * ct.sizeof(_lib.LoraAdapter), \
+            "table: the contiguous bytes of n_adapters qb200_lora_adapter entries"
+
+
+def _check_dora_norm(tables, mag_tables, stack_rows, rank_offsets, gram_offsets, rank_total, gram_total, packeds, n_out, k_in,
+                     row_norm2s, cdt, n_adapters, r):
+    n = len(tables)
+    assert 1 <= n <= 3 and len(mag_tables) == n and len(row_norm2s) == n and len(packeds) == n, \
+        "1..3 problems: one adapter table, magnitude table, base and row norm each"
+    _device(*tables, *mag_tables, stack_rows, rank_offsets, gram_offsets, *row_norm2s, *packeds)
+    _check_tables(tables, n_adapters)
+    for t in mag_tables:
+        assert t.dtype == torch.int64 and t.shape == (n_adapters,) and t.is_contiguous(), "magnitude table: int64 [n_adapters]"
+    for t in row_norm2s:
+        assert t.dtype == torch.float32 and t.shape == (n_out,) and t.is_contiguous(), "row norms: contiguous fp32 [N]"
+    assert stack_rows.dtype == torch.int32 and stack_rows.shape == (rank_total,) and stack_rows.is_contiguous(), \
+        "stack_rows: contiguous int32 [rank_total]"
+    for t in (rank_offsets, gram_offsets):
+        assert t.dtype == torch.int64 and t.shape == (n_adapters,) and t.is_contiguous(), "offsets: contiguous int64 [n_adapters]"
+    assert cdt in (torch.bfloat16, torch.float16), "compute dtype: bf16 or fp16"
+    assert 8 <= r <= F.LORA_MAX_RANK and r % 8 == 0 and rank_total >= 8 and gram_total >= 64, "R: a multiple of 8 in [8, 256]"
+    assert n_out % 8 == 0 and k_in % 8 == 0, "N and K: multiples of 8"
+
+
+@torch.library.custom_op("qlora_b200::dora_segmented_norm", mutates_args=())
+def dora_segmented_norm(tables: list[Tensor], mag_tables: list[Tensor], stack_rows: Tensor, rank_offsets: Tensor,
+                        gram_offsets: Tensor, rank_total: int, gram_total: int, packeds: list[Tensor], absmax: list[Tensor],
+                        code2: list[Optional[Tensor]], absmax2: list[Optional[Tensor]], offset: list[Optional[Tensor]], n_out: int,
+                        k_in: int, state_dtype: torch.dtype, row_norm2s: list[Tensor], cdt: torch.dtype, n_adapters: int,
+                        r: int) -> tuple[Tensor, Tensor]:
+    """(c, n), fp32 [P, n_adapters, N]: DoRA's detached norm n_a = ||W_p + s_a B_a A_a||_row and c_a = m_a / n_a of every
+    adapter of every problem, in a number of launches that does not depend on the adapters: `qb200_dora_stack_a` (each set's
+    A matrices as rank_total rows), one grouped fused forward P_p = A_stack_p . W_p^T with an fp32 output, and
+    `qb200_dora_norm_segmented` (the Gram matrices, then the per-row expansion of DESIGN.md §6b)."""
+    _check_dora_norm(tables, mag_tables, stack_rows, rank_offsets, gram_offsets, rank_total, gram_total, packeds, n_out, k_in,
+                     row_norm2s, cdt, n_adapters, r)
+    n = len(tables)
+    dev = packeds[0].device
+    a_st = torch.empty((n, rank_total, k_in), dtype=cdt, device=dev)
+    ps = torch.empty((n, rank_total, n_out), dtype=torch.float32, device=dev)
+    gram = torch.empty((n, gram_total), dtype=torch.float32, device=dev)
+    cs = torch.empty((n, n_adapters, n_out), dtype=torch.float32, device=dev)
+    nrms = torch.empty_like(cs)
+    lib = _lib.load()
+    dt = DTYPE_CODE[cdt]
+    tables_p = _ptrs(tables)
+    F.LAUNCH_COUNTER[0] += 3
+    with torch.cuda.device(dev):
+        check(lib.qb200_dora_stack_a(dt, n, tables_p, ptr(stack_rows), ptr(rank_offsets), rank_total, _ptrs(a_st.unbind(0)),
+                                     n_adapters, k_in, r, stream_ptr(dev)), "dora_stack_a")
+    nf4_linear_group(False, list(a_st.unbind(0)), packeds, absmax, code2, absmax2, offset, n_out, k_in, state_dtype, [], [], [],
+                     list(ps.unbind(0)), torch.float32, [], None, False)
+    with torch.cuda.device(dev):
+        check(lib.qb200_dora_norm_segmented(dt, n, tables_p, _ptrs(mag_tables), ptr(rank_offsets), ptr(gram_offsets), rank_total,
+                                            gram_total, _ptrs(ps.unbind(0)), _ptrs(row_norm2s), _ptrs(gram.unbind(0)),
+                                            _ptrs(cs.unbind(0)), _ptrs(nrms.unbind(0)), n_adapters, n_out, k_in, r, stream_ptr(dev)),
+              "dora_norm_segmented")
+    return cs, nrms
+
+
+@dora_segmented_norm.register_fake
+def _(tables, mag_tables, stack_rows, rank_offsets, gram_offsets, rank_total, gram_total, packeds, absmax, code2, absmax2, offset,
+      n_out, k_in, state_dtype, row_norm2s, cdt, n_adapters, r):
+    _check_dora_norm(tables, mag_tables, stack_rows, rank_offsets, gram_offsets, rank_total, gram_total, packeds, n_out, k_in,
+                     row_norm2s, cdt, n_adapters, r)
+    cs = row_norm2s[0].new_empty((len(tables), n_adapters, n_out))
+    return cs, torch.empty_like(cs)
+
+
+def _check_dora_fwd(xs, tables, rows, n_adapters, r, cs, outs, qs):
+    _check_segmented_fwd(xs, tables, rows, n_adapters, r, outs)
+    n, m, n_out = len(tables), xs[0].shape[0], outs[0].shape[1]
+    _device(cs, *qs)
+    assert cs.dtype == torch.float32 and cs.shape == (n, n_adapters, n_out) and cs.is_contiguous(), "c: contiguous fp32 [P, n, N]"
+    assert not qs or (len(qs) == n and len(xs) == n), "Q: one per problem, with one dropped input per problem"
+    for q in qs:
+        assert q.shape == (m, n_out) and q.dtype == xs[0].dtype and q.stride() == outs[0].stride(), "Q: of the outputs' layout"
+
+
+@torch.library.custom_op("qlora_b200::dora_segmented_fwd", mutates_args=("outs", "qs"))
+def dora_segmented_fwd(xs: list[Tensor], tables: list[Tensor], rows: Tensor, n_adapters: int, r: int, cs: Tensor,
+                       outs: list[Tensor], qs: list[Tensor]) -> tuple[Tensor, Tensor]:
+    """`lora_segmented_fwd` with DoRA's magnitude scale `cs` (fp32 [P, n, N], `dora_segmented_norm`) in the expand
+    (`qb200_dora_expand_segmented`): without dropout (`qs` empty) outs[p][t] = rn(c_a . (outs[p][t] + U_p[t] . B_a^T)); with
+    it outs[p][t] = rn(outs[p][t] + (c_a - 1) . Q_p[t] + c_a . U_p[t] . B_a^T), Q_p = rn(Q_p + U_p . B_a^T) in place, Q_p
+    given as rn(xs[p] . W_p^T).  Returns (U [P, M, r], the segment table's workspace)."""
+    _check_dora_fwd(xs, tables, rows, n_adapters, r, cs, outs, qs)
+    m = xs[0].shape[0]
+    dev = xs[0].device
+    us = torch.empty((len(tables), m, r), dtype=xs[0].dtype, device=dev)
+    ws = torch.empty(segment_workspace_bytes(m, n_adapters), dtype=torch.uint8, device=dev)
+    if m:
+        _segmented_add(xs, tables, rows, n_adapters, r, outs, list(us.unbind(0)), ws, dora=(cs, qs))
+    return us, ws
+
+
+@dora_segmented_fwd.register_fake
+def _(xs, tables, rows, n_adapters, r, cs, outs, qs):
+    _check_dora_fwd(xs, tables, rows, n_adapters, r, cs, outs, qs)
+    m = xs[0].shape[0]
+    return xs[0].new_empty((len(tables), m, r)), xs[0].new_empty((segment_workspace_bytes(m, n_adapters),), dtype=torch.uint8)
+
+
+def _check_dora_scale(g2ds, tables, rank_offsets, rank_total, qs, cs, nrms, ws, n_adapters, r, split):
+    n = len(tables)
+    assert 1 <= n <= 3 and len(g2ds) == n and len(qs) == n, "1..3 problems: one dY and one Q (or y) each"
+    _device(*g2ds, *tables, rank_offsets, *qs, cs, nrms, ws)
+    _check_tables(tables, n_adapters)
+    m, n_out = g2ds[0].shape
+    cdt = g2ds[0].dtype
+    assert cdt in (torch.bfloat16, torch.float16), "dY: bf16 or fp16"
+    for t in (*g2ds, *qs):
+        assert t.shape == (m, n_out) and t.dtype == cdt and t.is_contiguous(), f"dY, Q: contiguous {cdt} [{m}, {n_out}]"
+    for t in (cs, nrms):
+        assert t.dtype == torch.float32 and t.shape == (n, n_adapters, n_out) and t.is_contiguous(), "c, n: fp32 [P, n, N]"
+    assert rank_offsets.dtype == torch.int64 and rank_offsets.shape == (n_adapters,), "rank_offsets: int64 [n_adapters]"
+    assert 8 <= r <= F.LORA_MAX_RANK and r % 8 == 0 and rank_total >= 8 and n_out % 8 == 0, "R: a multiple of 8 in [8, 256]"
+    assert ws.dtype == torch.uint8 and ws.dim() == 1, "ws: the forward's segment table"
+    return m, n_out, cdt
+
+
+@torch.library.custom_op("qlora_b200::dora_grad_scale", mutates_args=())
+def dora_grad_scale(g2ds: list[Tensor], tables: list[Tensor], rank_offsets: Tensor, rank_total: int, qs: list[Tensor], cs: Tensor,
+                    nrms: Tensor, ws: Tensor, n_adapters: int, r: int, split: bool) -> tuple[Tensor, Tensor, Tensor]:
+    """`qb200_dora_grad_scale_segmented` over the forward's segment table: (dQ [P, M, N] = rn(dY . c_a), dD [P, M, N] =
+    rn(dY . (c_a - 1)) with `split` (else an empty tensor), dm [P, n . N] = rn(sum_t dY . Q / n_a) of the compute dtype).
+    `qs`: the expand's Q_p with `split`, else the forward's outputs y_p (Q = y / c)."""
+    m, n_out, cdt = _check_dora_scale(g2ds, tables, rank_offsets, rank_total, qs, cs, nrms, ws, n_adapters, r, split)
+    n = len(tables)
+    dev = g2ds[0].device
+    dq = torch.empty((n, m, n_out), dtype=cdt, device=dev)
+    dd = torch.empty((n, m, n_out) if split else (0,), dtype=cdt, device=dev)
+    dm = torch.empty((n, n_adapters * n_out), dtype=cdt, device=dev)
+    if m == 0:
+        return dq, dd, dm.zero_()
+    lib = _lib.load()
+    assert ws.numel() >= lib.qb200_lora_segment_workspace_size(m, n_adapters), "ws: the forward's segment table for these rows"
+    F.LAUNCH_COUNTER[0] += 1
+    with torch.cuda.device(dev):
+        check(lib.qb200_dora_grad_scale_segmented(DTYPE_CODE[cdt], n, int(split), _ptrs(tables), ptr(rank_offsets), rank_total,
+                                                  _ptrs(g2ds), _ptrs(qs), _ptrs(cs.unbind(0)), _ptrs(nrms.unbind(0)), n_out,
+                                                  _ptrs(dq.unbind(0)), _ptrs(dd.unbind(0)) if split else None, _ptrs(dm.unbind(0)),
+                                                  n_adapters, ptr(ws), ws.numel(), m, n_out, r, stream_ptr(dev)),
+              "dora_grad_scale_segmented")
+    return dq, dd, dm
+
+
+@dora_grad_scale.register_fake
+def _(g2ds, tables, rank_offsets, rank_total, qs, cs, nrms, ws, n_adapters, r, split):
+    m, n_out, cdt = _check_dora_scale(g2ds, tables, rank_offsets, rank_total, qs, cs, nrms, ws, n_adapters, r, split)
+    n, g = len(tables), g2ds[0]
+    return g.new_empty((n, m, n_out)), g.new_empty((n, m, n_out) if split else (0,)), g.new_empty((n, n_adapters * n_out))
+
+
+def _check_dora_bwd(dqs, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dxs):
+    n = len(tables)
+    m, k = xls[0].shape
+    _check_segmented_bwd(dqs, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, None, len(xls) > 1)
+    assert len(dxs) in (1, n) and (len(dxs) == 1) == (len(xls) == 1), "one dx (no dropout) or one dxd per problem"
+    for d in dxs:
+        assert d.shape == (m, k) and d.dtype == dqs[0].dtype and d.stride(1) == 1, f"dx: {dqs[0].dtype} [{m}, {k}] rows"
+    return m, dqs[0].shape[1], k, dqs[0].dtype
+
+
+@torch.library.custom_op("qlora_b200::dora_segmented_bwd", mutates_args=("dxs",))
+def dora_segmented_bwd(dqs: list[Tensor], tables: list[Tensor], rank_offsets: Tensor, rank_total: int, us: Tensor,
+                       xls: list[Tensor], ws: Tensor, n_adapters: int, r: int, dxs: list[Tensor]) -> tuple[Tensor, Tensor]:
+    """The adapters' part of a segmented DoRA backward, over dQ_p = rn(dY_p . c): G_p = rn(s_a . dQ_p . B_{p,a}); the input
+    term added in place to the base dX launches' outputs, dxs[0] += sum_p G_p . A_{p,a} (one shared input) or dxs[p] +=
+    G_p . A_{p,a} (one dropped input per problem), one rounding each; and the flat dA [P, rank_total . K] = G^T . xl and
+    dB [P, rank_total . N] = dQ^T . U, laid out as `lora_segmented_bwd`'s."""
+    m, n_out, k, cdt = _check_dora_bwd(dqs, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dxs)
+    n = len(tables)
+    dev = dqs[0].device
+    d_a = torch.empty((n, rank_total * k), dtype=cdt, device=dev)
+    d_b = torch.empty((n, rank_total * n_out), dtype=cdt, device=dev)
+    if m == 0:
+        return d_a.zero_(), d_b.zero_()
+    dqs = [g.contiguous() for g in dqs]
+    xls = [x.contiguous() for x in xls] * (n // len(xls))
+    gs = torch.empty((n, m, r), dtype=cdt, device=dev)
+    lib = _lib.load()
+    ws_bytes = ws.numel()
+    assert ws_bytes >= lib.qb200_lora_segment_workspace_size(m, n_adapters), "ws: the forward's segment table for these rows"
+    tables_p, gs_p = _ptrs(tables), _ptrs(gs.unbind(0))
+    dt = DTYPE_CODE[cdt]
+    F.LAUNCH_COUNTER[0] += 3 + len(dxs)
+    with torch.cuda.device(dev):
+        s = stream_ptr(dev)
+        check(lib.qb200_lora_grad_shrink_segmented(dt, n, _ptrs(dqs), n_out, tables_p, gs_p, r, n_adapters, ptr(ws), ws_bytes, m,
+                                                   n_out, r, s), "lora_grad_shrink_segmented")
+        if len(dxs) == 1:
+            check(lib.qb200_lora_grad_input_segmented(dt, n, 1, tables_p, gs_p, r, _ptrs(dxs * n), dxs[0].stride(0), n_adapters,
+                                                      ptr(ws), ws_bytes, m, k, r, s), "lora_grad_input_segmented")
+        else:
+            for p in range(n):
+                check(lib.qb200_lora_grad_input_segmented(dt, 1, 1, _ptrs(tables[p:p + 1]), _ptrs(gs[p:p + 1].unbind(0)), r,
+                                                          _ptrs(dxs[p:p + 1]), dxs[p].stride(0), n_adapters, ptr(ws), ws_bytes, m,
+                                                          k, r, s), "lora_grad_input_segmented")
+        check(lib.qb200_lora_weight_grad_segmented(dt, n, 0, tables_p, ptr(rank_offsets), rank_total, gs_p, r, _ptrs(xls), k,
+                                                   _ptrs(d_a.unbind(0)), n_adapters, ptr(ws), ws_bytes, m, k, r, s),
+              "lora_weight_grad_segmented")
+        check(lib.qb200_lora_weight_grad_segmented(dt, n, 1, tables_p, ptr(rank_offsets), rank_total, _ptrs(us.unbind(0)), r,
+                                                   _ptrs(dqs), n_out, _ptrs(d_b.unbind(0)), n_adapters, ptr(ws), ws_bytes, m,
+                                                   n_out, r, s), "lora_weight_grad_segmented")
+    return d_a, d_b
+
+
+@dora_segmented_bwd.register_fake
+def _(dqs, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dxs):
+    m, n_out, k, cdt = _check_dora_bwd(dqs, tables, rank_offsets, rank_total, us, xls, ws, n_adapters, r, dxs)
+    n = len(tables)
+    return dqs[0].new_empty((n, rank_total * k)), dqs[0].new_empty((n, rank_total * n_out))
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -16,6 +16,12 @@
 // All are one warpgroup of wgmma m64n128k16 (bf16 or fp16 in, fp32 accumulate) per 64-row x 128-column tile, with the next
 // 64-wide contraction chunk loaded into registers while the current one is multiplied.  grid.z is the problem of a
 // grouped launch (q/k/v, gate/up): each problem has its own adapter table and U, and all share the segment table.
+// DoRA over the same tables (DESIGN.md §6e):
+//   dora_gather_a_kernel        every adapter's A stacked into [sum r, K] rows, the input of one fused forward P = A . W^T.
+//   dora_gram_kernel            G_a = A_a . A_a^T per adapter, fp32.
+//   dora_norm_kernel            n_a = sqrt(||W_f||^2 + 2 s B_a P_a + s^2 B_a G_a B_a^T) and c_a = m_a / n_a per row f, fp32.
+//   lora_segmented_kernel<kDora> the expand with DoRA's magnitude scale in the epilogue.
+//   dora_grad_scale_kernel      dQ = rn(dY . c_a), dD = rn(dY . (c_a - 1)) and dm_a = rn(sum_t dY . Q / n_a) per bucket.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -151,6 +157,13 @@ struct Problems {
   void* out[kMaxProb];
 };
 
+// The expand's DoRA operands, per problem: c [n, N] fp32 and (dropout) Q [M, N], read as rn(xd . W^T) and overwritten with
+// the pre-scale term rn(Qb + U . B_a^T); its row pitch is the output's.
+struct DoraProblems : Problems {
+  const float* c[kMaxProb];
+  void* q[kMaxProb];
+};
+
 // element z of a kernel-parameter array, without copying the array to local memory as a dynamic index would
 template <typename T>
 __device__ __forceinline__ T pick(const T (&v)[kMaxProb], int z) {
@@ -166,9 +179,13 @@ __device__ __forceinline__ T pick(const T (&v)[kMaxProb], int z) {
 // so every chunk runs all four and no data-dependent branch sits between them.
 // Every row index comes from the segment table and is checked against [0, M); an adapter index outside [0, n), an entry whose
 // rank is not a positive multiple of 8, or (expand) a clamped rank of 0 makes the tile write nothing.
-template <typename T16, bool kShrink>
-__global__ void __launch_bounds__(kThreads) lora_segmented_kernel(Problems p, const uint8_t* __restrict__ ws, int64_t ld_x,
+// kDora (expand only; DoRA's magnitude scale c = c_a[column] of the tile's adapter, C = U . B_a^T in fp32):
+//   1: y = rn(c . (y + C));   2 (dropout): y = rn(y + (c - 1) . Qb + c . C) and Q = rn(Qb + C) in place of Qb.
+template <typename T16, bool kShrink, int kDora = 0>
+__global__ void __launch_bounds__(kThreads) lora_segmented_kernel(std::conditional_t<(kDora != 0), DoraProblems, Problems> p,
+                                                                  const uint8_t* __restrict__ ws, int64_t ld_x,
                                                                   int64_t ld_out, int M, int n, int N, int K, int R) {
+  static_assert(kDora == 0 || !kShrink, "DoRA scales the expand only");
   __shared__ __align__(1024) uint4 sX[kTileM * kChunk / 8];
   __shared__ __align__(1024) uint4 sO[kTileN * kChunk / 8];
   __shared__ int s_row[kTileM];
@@ -264,6 +281,19 @@ __global__ void __launch_bounds__(kThreads) lora_segmented_kernel(Problems p, co
       const float s0 = acc[4 * j + 2 * h], s1 = acc[4 * j + 2 * h + 1];
       if constexpr (kShrink) {
         *dst = c < rank ? round16x2<T16>(s0 * ad.scale, s1 * ad.scale) : 0u;
+      } else if constexpr (kDora != 0) {
+        const float2 cc = *reinterpret_cast<const float2*>(pick(p.c, z) + int64_t(a) * N + c);
+        uint32_t y = *dst;
+        const float2 f = widen2(*reinterpret_cast<const T2*>(&y));
+        if constexpr (kDora == 1) {
+          *dst = round16x2<T16>(cc.x * (f.x + s0), cc.y * (f.y + s1));
+        } else {
+          uint32_t* qdst = reinterpret_cast<uint32_t*>(static_cast<T16*>(pick(p.q, z)) + int64_t(t) * ld_out + c);
+          uint32_t qv = *qdst;
+          const float2 qb = widen2(*reinterpret_cast<const T2*>(&qv));
+          *dst = round16x2<T16>(f.x + (cc.x - 1.0f) * qb.x + cc.x * s0, f.y + (cc.y - 1.0f) * qb.y + cc.y * s1);
+          *qdst = round16x2<T16>(qb.x + s0, qb.y + s1);
+        }
       } else {
         uint32_t y = *dst;
         const float2 f = widen2(*reinterpret_cast<const T2*>(&y));
@@ -540,8 +570,267 @@ __global__ void __launch_bounds__(kThreads) lora_weight_grad_kernel(WgradProblem
   }
 }
 
+// ---- DoRA ---------------------------------------------------------------------------------------------------------------
+// An adapter's entry is usable when its rank is a positive multiple of 8 whose clamped rank is not 0 and its rank offset keeps
+// [off, off + rank) inside [0, total); the kernels below treat the rows and outputs of any other adapter as the base's.
+__device__ __forceinline__ int dora_rank(const qb200_lora_adapter& ad, const int64_t* rank_off, int a, int64_t total, int R,
+                                         int64_t& off) {
+  if (ad.rank <= 0 || (ad.rank & 7)) return 0;
+  const int rank = MixedLora::rank(ad, R);
+  off = rank_off[a];
+  return (off < 0 || off > total - rank) ? 0 : rank;
+}
+
+// out_p[j, :] = A_{p,a}[j - off_a, :] for every stacked row j of adapter a = stack_rows[j]; zeros for a row that lies
+// outside its adapter's clamped rank.  One CTA per (stacked row, problem), 16 bytes per thread per step.
+struct GatherProblems {
+  const qb200_lora_adapter* table[kMaxProb];
+  void* out[kMaxProb];
+};
+__global__ void __launch_bounds__(kThreads) dora_gather_a_kernel(GatherProblems p, const int32_t* __restrict__ stack_rows,
+                                                                 const int64_t* __restrict__ rank_off, int64_t total, int n, int K,
+                                                                 int R) {
+  ptx::grid_dep_launch();
+  ptx::grid_dep_wait();
+  const int64_t j = blockIdx.x;
+  const int z = blockIdx.z;
+  const int a = stack_rows[j];
+  const uint4* src = nullptr;
+  if (a >= 0 && a < n) {
+    const qb200_lora_adapter ad = pick(p.table, z)[a];
+    int64_t off = 0;
+    const int rank = dora_rank(ad, rank_off, a, total, R, off);
+    if (j >= off && j - off < rank) src = reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(ad.A) + (j - off) * K);
+  }
+  uint4* dst = reinterpret_cast<uint4*>(static_cast<uint16_t*>(pick(p.out, z)) + j * K);
+  for (int v = threadIdx.x; v < K / 8; v += kThreads) dst[v] = src ? __ldg(src + v) : make_uint4(0, 0, 0, 0);
+}
+
+// G_a = A_a . A_a^T [r_a, r_a] row-major at gram_off[a] of problem z's fp32 buffer (an offset that would write past gram_total
+// writes nothing).  One CTA of 256 threads per (adapter, 64 x 64 tile, problem), 4 x 4 outputs per thread, K in chunks of 32
+// summed in order.
+constexpr int kGramTile = 64, kGramChunk = 32, kGramThreads = 256;
+struct NormProblems {
+  const qb200_lora_adapter* table[kMaxProb];
+  const void* const* mag[kMaxProb];    // DEVICE: n pointers to each adapter's magnitude [N]
+  const float* P[kMaxProb];            // [total, N]: row off_a + j is A_a[j] . W^T
+  const float* norm2[kMaxProb];        // ||W_f||^2 [N]
+  float* gram[kMaxProb];               // sum_a r_a^2
+  float* c[kMaxProb];                  // [n, N]
+  float* nrm[kMaxProb];                // [n, N]
+};
+template <typename T16>
+__device__ __forceinline__ float h2f(uint16_t h) {
+  if constexpr (std::is_same_v<T16, __half>) return __half2float(__ushort_as_half(h));
+  else return __uint_as_float(uint32_t(h) << 16);
+}
+template <typename T16>
+__device__ __forceinline__ uint16_t f2h(float f) {
+  if constexpr (std::is_same_v<T16, __half>) return __half_as_ushort(__float2half_rn(f));
+  else return __bfloat16_as_ushort(__float2bfloat16_rn(f));
+}
+
+template <typename T16>
+__global__ void __launch_bounds__(kGramThreads) dora_gram_kernel(NormProblems p, const int64_t* __restrict__ rank_off,
+                                                                 const int64_t* __restrict__ gram_off, int64_t total,
+                                                                 int64_t gram_total, int n, int K, int R) {
+  __shared__ float sI[kGramChunk][kGramTile + 1];
+  __shared__ float sJ[kGramChunk][kGramTile + 1];
+  ptx::grid_dep_launch();
+  ptx::grid_dep_wait();
+  const int rt = (R + kGramTile - 1) / kGramTile;
+  const int a = int(blockIdx.x / unsigned(rt * rt)), tile = int(blockIdx.x % unsigned(rt * rt));
+  const int i0 = (tile / rt) * kGramTile, j0 = (tile % rt) * kGramTile, z = blockIdx.z;
+  if (a >= n) return;
+  const qb200_lora_adapter ad = pick(p.table, z)[a];
+  int64_t off = 0;
+  const int rank = dora_rank(ad, rank_off, a, total, R, off);
+  if (i0 >= rank || j0 >= rank) return;
+  const int64_t g0 = gram_off[a];
+  if (g0 < 0 || g0 > gram_total - int64_t(rank) * rank) return;
+  const uint16_t* A = static_cast<const uint16_t*>(ad.A);
+  const int tid = threadIdx.x, ty = tid / 16, tx = tid % 16;
+  float acc[4][4] = {};
+  for (int k0 = 0; k0 < K; k0 += kGramChunk) {
+#pragma unroll
+    for (int e = 0; e < kGramTile * kGramChunk / kGramThreads; ++e) {
+      const int v = tid + e * kGramThreads, r = v / kGramChunk, k = v % kGramChunk;
+      const int ri = i0 + r, rj = j0 + r;
+      sI[k][r] = ri < rank && k0 + k < K ? h2f<T16>(A[int64_t(ri) * K + k0 + k]) : 0.0f;
+      sJ[k][r] = rj < rank && k0 + k < K ? h2f<T16>(A[int64_t(rj) * K + k0 + k]) : 0.0f;
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int k = 0; k < kGramChunk; ++k) {
+      float vi[4], vj[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) vi[u] = sI[k][ty * 4 + u], vj[u] = sJ[k][tx * 4 + u];
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+#pragma unroll
+        for (int w = 0; w < 4; ++w) acc[u][w] = fmaf(vi[u], vj[w], acc[u][w]);
+    }
+    __syncthreads();
+  }
+  float* g = pick(p.gram, z) + g0;
+#pragma unroll
+  for (int u = 0; u < 4; ++u)
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const int i = i0 + ty * 4 + u, j = j0 + tx * 4 + w;
+      if (i < rank && j < rank) g[int64_t(i) * rank + j] = acc[u][w];
+    }
+}
+
+// n_a[f]^2 = ||W_f||^2 + 2 s_a sum_j B_a[f, j] P[off_a + j, f] + s_a^2 sum_{j,k} B_a[f, j] G_a[j, k] B_a[f, k], clamped at 0;
+// c_a[f] = m_a[f] / n_a[f].  One CTA of 256 threads per (adapter, 64 rows f, problem): four threads per row, thread q taking
+// the j (cross term) and k (quadratic term) congruent to q mod 4, reduced in a fixed order.  An unusable adapter gets c = n = 0.
+constexpr int kNormRows = 64, kNormGRows = 8;
+template <typename T16>
+__global__ void __launch_bounds__(kGramThreads) dora_norm_kernel(NormProblems p, const int64_t* __restrict__ rank_off,
+                                                                 const int64_t* __restrict__ gram_off, int64_t total,
+                                                                 int64_t gram_total, int n, int N, int R) {
+  __shared__ uint16_t sB[kNormRows][kMaxLoraRank + 8];
+  __shared__ float sG[kNormGRows][kMaxLoraRank];
+  ptx::grid_dep_launch();
+  ptx::grid_dep_wait();
+  const int a = blockIdx.x, f0 = blockIdx.y * kNormRows, z = blockIdx.z;
+  const int tid = threadIdx.x, q = tid & 3, fl = tid >> 2, f = f0 + fl;
+  const qb200_lora_adapter ad = pick(p.table, z)[a];
+  int64_t off = 0;
+  int rank = dora_rank(ad, rank_off, a, total, R, off);
+  const int64_t g0 = gram_off[a];
+  if (rank && (g0 < 0 || g0 > gram_total - int64_t(rank) * rank)) rank = 0;
+  float* c_out = pick(p.c, z) + int64_t(a) * N;
+  float* n_out = pick(p.nrm, z) + int64_t(a) * N;
+  if (rank == 0) {
+    if (q == 0 && f < N) c_out[f] = 0.0f, n_out[f] = 0.0f;
+    return;
+  }
+  const uint16_t* B = static_cast<const uint16_t*>(ad.B);
+  for (int v = tid; v < kNormRows * rank; v += kGramThreads) {
+    const int r = v / rank, k = v % rank;
+    sB[r][k] = f0 + r < N ? B[int64_t(f0 + r) * ad.rank + k] : uint16_t(0);
+  }
+  __syncthreads();
+  const bool live = f < N;
+  const float* P = pick(p.P, z) + off * N;
+  float cross = 0.0f;
+  if (live)
+    for (int j = q; j < rank; j += 4) cross = fmaf(h2f<T16>(sB[fl][j]), P[int64_t(j) * N + f], cross);
+  const float* G = pick(p.gram, z) + g0;
+  float quad = 0.0f;
+  for (int j0 = 0; j0 < rank; j0 += kNormGRows) {
+    for (int v = tid; v < kNormGRows * rank; v += kGramThreads) {
+      const int r = v / rank, k = v % rank;
+      sG[r][k] = j0 + r < rank ? G[int64_t(j0 + r) * rank + k] : 0.0f;
+    }
+    __syncthreads();
+    if (live) {
+#pragma unroll
+      for (int jj = 0; jj < kNormGRows; ++jj) {
+        float h = 0.0f;
+        for (int k = q; k < rank; k += 4) h = fmaf(sG[jj][k], h2f<T16>(sB[fl][k]), h);
+        if (j0 + jj < rank) quad = fmaf(h2f<T16>(sB[fl][j0 + jj]), h, quad);
+      }
+    }
+    __syncthreads();
+  }
+  cross += __shfl_xor_sync(0xffffffffu, cross, 1);
+  cross += __shfl_xor_sync(0xffffffffu, cross, 2);
+  quad += __shfl_xor_sync(0xffffffffu, quad, 1);
+  quad += __shfl_xor_sync(0xffffffffu, quad, 2);
+  if (!live || q != 0) return;
+  const float s = ad.scale;
+  const float n2 = fmaxf(pick(p.norm2, z)[f] + (2.0f * s) * cross + (s * s) * quad, 0.0f);
+  const float nrm = sqrtf(n2);
+  const uint16_t* mag = static_cast<const uint16_t*>(pick(p.mag, z)[a]);
+  c_out[f] = (mag ? h2f<T16>(mag[f]) : 0.0f) / nrm;
+  n_out[f] = nrm;
+}
+
+// Per bucket b (an adapter, or b = n: the rows without one) and problem, over the bucket's sorted rows t, columns f:
+//   dQ[t] = rn(dY[t] . c_a),  kDropout: dD[t] = rn(dY[t] . (c_a - 1)),  dm_a = rn(sum_t dY[t] . Q[t] / n_a)
+// where Q is the expand's pre-scale output (kDropout) or y / c_a (no dropout; an element with c = 0 adds nothing).  Rows
+// without a usable adapter copy dY into dQ and write dD = 0; an adapter without rows gets dm = 0.  One CTA of 256 threads
+// per (bucket, 64 columns, problem): eight row groups of 32 threads x 2 columns, row i of the bucket to group i % 8, the
+// groups' fp32 sums added in group order.
+struct ScaleProblems {
+  const qb200_lora_adapter* table[kMaxProb];
+  const void* dy[kMaxProb];
+  const void* q[kMaxProb];             // Q (dropout) or y, row pitch ld
+  const float* c[kMaxProb];            // [n, N]
+  const float* nrm[kMaxProb];          // [n, N]
+  void* dq[kMaxProb];
+  void* dd[kMaxProb];
+  void* dm[kMaxProb];                  // [n, N] of the compute dtype
+};
+constexpr int kScaleCols = 64, kScaleGroups = 8;
+template <typename T16, bool kDropout>
+__global__ void __launch_bounds__(kGramThreads) dora_grad_scale_kernel(ScaleProblems p, const int64_t* __restrict__ rank_off,
+                                                                       int64_t total, const uint8_t* __restrict__ ws, int64_t ld,
+                                                                       int M, int n, int N, int R) {
+  __shared__ float2 s_part[kScaleGroups][kScaleCols / 2];
+  ptx::grid_dep_launch();
+  ptx::grid_dep_wait();
+  const int b = blockIdx.x, z = blockIdx.z;
+  const int tid = threadIdx.x, g = tid >> 5, col = blockIdx.y * kScaleCols + 2 * (tid & 31);
+  const Layout L = layout(M, n);
+  const int* perm = reinterpret_cast<const int*>(ws + L.perm);
+  const int* boff = reinterpret_cast<const int*>(ws + L.off);
+  const int b0 = max(0, min(boff[b], M)), b1 = max(b0, min(boff[b + 1], M));
+  int rank = 0;
+  if (b < n) {
+    int64_t off = 0;
+    rank = dora_rank(pick(p.table, z)[b], rank_off, b, total, R, off);
+  }
+  using T2 = typename Vec2<T16>::type;
+  const bool live = col < N;
+  float2 cc = make_float2(1.0f, 1.0f), acc = make_float2(0.0f, 0.0f);
+  if (rank && live) cc = *reinterpret_cast<const float2*>(pick(p.c, z) + int64_t(b) * N + col);
+  const T16* dy = static_cast<const T16*>(pick(p.dy, z));
+  const T16* qy = static_cast<const T16*>(pick(p.q, z));
+  T16* dq = static_cast<T16*>(pick(p.dq, z));
+  T16* dd = static_cast<T16*>(pick(p.dd, z));
+  if (live) {
+    for (int i = b0 + g; i < b1; i += kScaleGroups) {
+      const int t = perm[i];
+      if (t < 0 || t >= M) continue;
+      const int64_t e = int64_t(t) * ld + col;
+      const uint32_t dv = *reinterpret_cast<const uint32_t*>(dy + e);
+      if (!rank) {
+        *reinterpret_cast<uint32_t*>(dq + e) = dv;
+        if (kDropout) *reinterpret_cast<uint32_t*>(dd + e) = 0u;
+        continue;
+      }
+      const float2 d = widen2(*reinterpret_cast<const T2*>(&dv));
+      const uint32_t qv = *reinterpret_cast<const uint32_t*>(qy + e);
+      float2 qf = widen2(*reinterpret_cast<const T2*>(&qv));
+      if (!kDropout) qf = make_float2(cc.x != 0.0f ? qf.x / cc.x : 0.0f, cc.y != 0.0f ? qf.y / cc.y : 0.0f);
+      *reinterpret_cast<uint32_t*>(dq + e) = round16x2<T16>(d.x * cc.x, d.y * cc.y);
+      if (kDropout) *reinterpret_cast<uint32_t*>(dd + e) = round16x2<T16>(d.x * (cc.x - 1.0f), d.y * (cc.y - 1.0f));
+      acc.x = fmaf(d.x, qf.x, acc.x);
+      acc.y = fmaf(d.y, qf.y, acc.y);
+    }
+  }
+  if (b >= n) return;
+  s_part[g][tid & 31] = acc;
+  __syncthreads();
+  if (g != 0 || !live) return;
+  float2 sum = s_part[0][tid];
+#pragma unroll
+  for (int k = 1; k < kScaleGroups; ++k) sum.x += s_part[k][tid].x, sum.y += s_part[k][tid].y;
+  uint32_t out = 0u;
+  if (rank && b1 > b0) {
+    const float2 nv = *reinterpret_cast<const float2*>(pick(p.nrm, z) + int64_t(b) * N + col);
+    out = round16x2<T16>(sum.x / nv.x, sum.y / nv.y);
+  }
+  *reinterpret_cast<uint32_t*>(static_cast<T16*>(pick(p.dm, z)) + int64_t(b) * N + col) = out;
+}
+
 }  // namespace seg
 }  // namespace qb200
+
 
 using namespace qb200;
 
@@ -761,4 +1050,174 @@ extern "C" int qb200_lora_weight_grad_segmented(int dtype, int nprob, int transp
                           ld_p, ld_q, m, n_adapters, d, r)
              : launch_pdl(seg::lora_weight_grad_kernel<__nv_bfloat16, false>, grid, seg::kThreads, 0, s, what, w, rank_offsets,
                           rank_total, ws, ld_p, ld_q, m, n_adapters, d, r);
+}
+
+// ---- DoRA entry points --------------------------------------------------------------------------------------------------
+// The checks the DoRA entry points share: dtype, problem count, adapter count, R and the per-problem tables.
+static int dora_args(const char* what, int dtype, int nprob, const qb200_lora_adapter* const* tables, int n_adapters, int64_t R) {
+  char msg[160];
+  if (dtype != QB200_DTYPE_BF16 && dtype != QB200_DTYPE_F16) {
+    snprintf(msg, sizeof(msg), "%s: dtype must be 2 (bf16) or 1 (fp16)", what);
+    return set_error(QB200_EINVAL, msg);
+  }
+  if (nprob < 1 || nprob > seg::kMaxProb || !tables) {
+    snprintf(msg, sizeof(msg), "%s: 1..3 problems and no null pointer", what);
+    return set_error(QB200_EINVAL, msg);
+  }
+  if (n_adapters < 1) {
+    snprintf(msg, sizeof(msg), "%s: n_adapters must be positive", what);
+    return set_error(QB200_EINVAL, msg);
+  }
+  if (R < 8 || R > kMaxLoraRank || R % 8 != 0) {
+    snprintf(msg, sizeof(msg), "%s: R must be a multiple of 8 in [8, 256]", what);
+    return set_error(QB200_EUNSUPPORTED, msg);
+  }
+  for (int i = 0; i < nprob; ++i) {
+    if (!tables[i]) {
+      snprintf(msg, sizeof(msg), "%s: null pointer", what);
+      return set_error(QB200_EINVAL, msg);
+    }
+    if (reinterpret_cast<uintptr_t>(tables[i]) % 8) {
+      snprintf(msg, sizeof(msg), "%s: tables must be 8-byte aligned", what);
+      return set_error(QB200_EINVAL, msg);
+    }
+  }
+  return 0;
+}
+
+// every pointer of a per-problem array present and `align`-byte aligned
+template <typename T>
+static bool all_set(const T* const* v, int nprob, int align) {
+  if (!v) return false;
+  for (int i = 0; i < nprob; ++i)
+    if (!v[i] || reinterpret_cast<uintptr_t>(v[i]) % align) return false;
+  return true;
+}
+
+extern "C" int qb200_dora_stack_a(int dtype, int nprob, const qb200_lora_adapter* const* tables, const int32_t* stack_rows,
+                                  const int64_t* rank_offsets, int64_t rank_total, void* const* out, int n_adapters, int64_t K,
+                                  int64_t R, void* stream) {
+  const char* what = "dora_stack_a";
+  int rc = dora_args(what, dtype, nprob, tables, n_adapters, R);
+  if (rc) return rc;
+  if (!stack_rows || !rank_offsets || !all_set(out, nprob, 16))
+    return set_error(QB200_EINVAL, "dora_stack_a: null pointer, or an output that is not 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(rank_offsets) % 8 || reinterpret_cast<uintptr_t>(stack_rows) % 4)
+    return set_error(QB200_EINVAL, "dora_stack_a: rank_offsets must be 8-byte and stack_rows 4-byte aligned");
+  if (K < 8 || K % 8 != 0 || K > INT32_MAX || rank_total < 8 || rank_total > INT32_MAX)
+    return set_error(QB200_EINVAL, "dora_stack_a: bad shape");
+  seg::GatherProblems p{};
+  for (int i = 0; i < nprob; ++i) p.table[i] = tables[i], p.out[i] = out[i];
+  const dim3 grid(unsigned(rank_total), 1, unsigned(nprob));
+  return launch_pdl(seg::dora_gather_a_kernel, grid, seg::kThreads, 0, static_cast<cudaStream_t>(stream), what, p, stack_rows,
+                    rank_offsets, rank_total, n_adapters, int(K), int(R));
+}
+
+extern "C" int qb200_dora_norm_segmented(int dtype, int nprob, const qb200_lora_adapter* const* tables, const void* const* mag_tables,
+                                         const int64_t* rank_offsets, const int64_t* gram_offsets, int64_t rank_total,
+                                         int64_t gram_total, const float* const* P, const float* const* row_norm2,
+                                         float* const* gram, float* const* c, float* const* norm, int n_adapters, int64_t N,
+                                         int64_t K, int64_t R, void* stream) {
+  const char* what = "dora_norm_segmented";
+  int rc = dora_args(what, dtype, nprob, tables, n_adapters, R);
+  if (rc) return rc;
+  if (!rank_offsets || !gram_offsets || !all_set(mag_tables, nprob, 8) || !all_set(P, nprob, 4) || !all_set(row_norm2, nprob, 4) ||
+      !all_set(gram, nprob, 4) || !all_set(c, nprob, 8) || !all_set(norm, nprob, 8))
+    return set_error(QB200_EINVAL, "dora_norm_segmented: null pointer, or c / norm not 8-byte and the other arrays not 4-byte aligned");
+  if (reinterpret_cast<uintptr_t>(rank_offsets) % 8 || reinterpret_cast<uintptr_t>(gram_offsets) % 8)
+    return set_error(QB200_EINVAL, "dora_norm_segmented: rank_offsets and gram_offsets must be 8-byte aligned");
+  const int64_t rt = (R + seg::kGramTile - 1) / seg::kGramTile;
+  if (N < 8 || N % 8 != 0 || N > INT32_MAX || (N + seg::kNormRows - 1) / seg::kNormRows > 65535 || K < 8 || K > INT32_MAX ||
+      int64_t(n_adapters) * rt * rt > INT32_MAX || rank_total < 8 || gram_total < 64)
+    return set_error(QB200_EINVAL, "dora_norm_segmented: bad shape");
+  seg::NormProblems p{};
+  for (int i = 0; i < nprob; ++i) {
+    p.table[i] = tables[i];
+    p.mag[i] = static_cast<const void* const*>(mag_tables[i]);
+    p.P[i] = P[i], p.norm2[i] = row_norm2[i], p.gram[i] = gram[i], p.c[i] = c[i], p.nrm[i] = norm[i];
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bool f16 = dtype == QB200_DTYPE_F16;
+  const dim3 g_grid(unsigned(n_adapters * rt * rt), 1, unsigned(nprob));
+  rc = f16 ? launch_pdl(seg::dora_gram_kernel<__half>, g_grid, seg::kGramThreads, 0, s, what, p, rank_offsets, gram_offsets,
+                        rank_total, gram_total, n_adapters, int(K), int(R))
+           : launch_pdl(seg::dora_gram_kernel<__nv_bfloat16>, g_grid, seg::kGramThreads, 0, s, what, p, rank_offsets, gram_offsets,
+                        rank_total, gram_total, n_adapters, int(K), int(R));
+  if (rc) return rc;
+  const dim3 n_grid(unsigned(n_adapters), unsigned((N + seg::kNormRows - 1) / seg::kNormRows), unsigned(nprob));
+  return f16 ? launch_pdl(seg::dora_norm_kernel<__half>, n_grid, seg::kGramThreads, 0, s, what, p, rank_offsets, gram_offsets,
+                          rank_total, gram_total, n_adapters, int(N), int(R))
+             : launch_pdl(seg::dora_norm_kernel<__nv_bfloat16>, n_grid, seg::kGramThreads, 0, s, what, p, rank_offsets, gram_offsets,
+                          rank_total, gram_total, n_adapters, int(N), int(R));
+}
+
+extern "C" int qb200_dora_expand_segmented(int dtype, int nprob, int dropout, const qb200_lora_adapter* const* tables,
+                                           const void* const* U, int64_t ld_u, const float* const* c, void* const* Q,
+                                           void* const* out, int64_t ld_out, int n_adapters, const void* workspace,
+                                           int64_t workspace_bytes, int64_t M, int64_t N, int64_t R, void* stream) {
+  const char* what = "dora_expand_segmented";
+  if (dropout != 0 && dropout != 1) return set_error(QB200_EINVAL, "dora_expand_segmented: dropout must be 0 or 1");
+  seg::DoraProblems p{};
+  int rc = segmented_args(what, dtype, nprob, tables, U, out, n_adapters, workspace, workspace_bytes, M, R, p);
+  if (rc) return rc;
+  if (!all_set(c, nprob, 8) || (dropout && !all_set(Q, nprob, 4)))
+    return set_error(QB200_EINVAL, "dora_expand_segmented: null pointer, or c not 8-byte or Q not 4-byte aligned");
+  if (N < 8 || N % 8 != 0 || N > INT32_MAX || int64_t(N + seg::kTileN - 1) / seg::kTileN > 65535)
+    return set_error(QB200_EINVAL, "dora_expand_segmented: bad shape");
+  if (ld_u == 0) ld_u = R;
+  if (ld_out == 0) ld_out = N;
+  if (ld_u < R || ld_u % 8 != 0 || ld_out < N || ld_out % 2 != 0)
+    return set_error(QB200_EINVAL, "dora_expand_segmented: bad row pitch");
+  for (int i = 0; i < nprob; ++i) p.c[i] = c[i], p.q[i] = dropout ? Q[i] : nullptr;
+  const dim3 grid(unsigned(seg::layout(M, n_adapters).n_tiles), unsigned((N + seg::kTileN - 1) / seg::kTileN), unsigned(nprob));
+  const auto* ws = static_cast<const uint8_t*>(workspace);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int m = int(M), n = n_adapters, nn = int(N), r = int(R);
+  if (dtype == QB200_DTYPE_F16)
+    return dropout ? launch_pdl(seg::lora_segmented_kernel<__half, false, 2>, grid, seg::kThreads, 0, s, what, p, ws, ld_u, ld_out, m, n,
+                                nn, 0, r)
+                   : launch_pdl(seg::lora_segmented_kernel<__half, false, 1>, grid, seg::kThreads, 0, s, what, p, ws, ld_u, ld_out, m, n,
+                                nn, 0, r);
+  return dropout ? launch_pdl(seg::lora_segmented_kernel<__nv_bfloat16, false, 2>, grid, seg::kThreads, 0, s, what, p, ws, ld_u, ld_out,
+                              m, n, nn, 0, r)
+                 : launch_pdl(seg::lora_segmented_kernel<__nv_bfloat16, false, 1>, grid, seg::kThreads, 0, s, what, p, ws, ld_u, ld_out,
+                              m, n, nn, 0, r);
+}
+
+extern "C" int qb200_dora_grad_scale_segmented(int dtype, int nprob, int dropout, const qb200_lora_adapter* const* tables,
+                                               const int64_t* rank_offsets, int64_t rank_total, const void* const* dY,
+                                               const void* const* Q, const float* const* c, const float* const* norm, int64_t ld,
+                                               void* const* dQ, void* const* dD, void* const* dm, int n_adapters,
+                                               const void* workspace, int64_t workspace_bytes, int64_t M, int64_t N, int64_t R,
+                                               void* stream) {
+  const char* what = "dora_grad_scale_segmented";
+  if (dropout != 0 && dropout != 1) return set_error(QB200_EINVAL, "dora_grad_scale_segmented: dropout must be 0 or 1");
+  seg::Problems base{};
+  int rc = segmented_args(what, dtype, nprob, tables, dY, dQ, n_adapters, workspace, workspace_bytes, M, R, base);
+  if (rc) return rc;
+  if (!rank_offsets || !all_set(Q, nprob, 4) || !all_set(c, nprob, 8) || !all_set(norm, nprob, 8) || !all_set(dm, nprob, 4) ||
+      (dropout && !all_set(dD, nprob, 4)) || reinterpret_cast<uintptr_t>(rank_offsets) % 8)
+    return set_error(QB200_EINVAL, "dora_grad_scale_segmented: null pointer or misaligned array");
+  if (N < 8 || N % 8 != 0 || N > INT32_MAX || (N + seg::kScaleCols - 1) / seg::kScaleCols > 65535 || rank_total < 8)
+    return set_error(QB200_EINVAL, "dora_grad_scale_segmented: bad shape");
+  if (ld == 0) ld = N;
+  if (ld < N || ld % 2 != 0) return set_error(QB200_EINVAL, "dora_grad_scale_segmented: bad row pitch");
+  seg::ScaleProblems p{};
+  for (int i = 0; i < nprob; ++i) {
+    p.table[i] = tables[i], p.dy[i] = dY[i], p.q[i] = Q[i], p.c[i] = c[i], p.nrm[i] = norm[i];
+    p.dq[i] = dQ[i], p.dd[i] = dropout ? dD[i] : nullptr, p.dm[i] = dm[i];
+  }
+  const dim3 grid(unsigned(n_adapters + 1), unsigned((N + seg::kScaleCols - 1) / seg::kScaleCols), unsigned(nprob));
+  const auto* ws = static_cast<const uint8_t*>(workspace);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int m = int(M), n = n_adapters, nn = int(N), r = int(R);
+  if (dtype == QB200_DTYPE_F16)
+    return dropout ? launch_pdl(seg::dora_grad_scale_kernel<__half, true>, grid, seg::kGramThreads, 0, s, what, p, rank_offsets,
+                                rank_total, ws, ld, m, n, nn, r)
+                   : launch_pdl(seg::dora_grad_scale_kernel<__half, false>, grid, seg::kGramThreads, 0, s, what, p, rank_offsets,
+                                rank_total, ws, ld, m, n, nn, r);
+  return dropout ? launch_pdl(seg::dora_grad_scale_kernel<__nv_bfloat16, true>, grid, seg::kGramThreads, 0, s, what, p, rank_offsets,
+                              rank_total, ws, ld, m, n, nn, r)
+                 : launch_pdl(seg::dora_grad_scale_kernel<__nv_bfloat16, false>, grid, seg::kGramThreads, 0, s, what, p, rank_offsets,
+                              rank_total, ws, ld, m, n, nn, r);
 }

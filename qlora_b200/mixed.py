@@ -27,7 +27,8 @@ with the sum rounded once, as `lora_linear4bit` does, except on the segmented pa
 
 Inference only, as in peft: a call in grad mode with an input or adapter weight that requires grad raises.  Dropout is the
 identity.  Training takes `lora_linear4bit_group_multi` / `lora_linear4bit_multi` (end of this file): the segmented forward
-at every token count, differentiable in the input and every adapter's weights (DESIGN.md §6d).  The compute dtype is the base's (bf16, or fp16 for `compute_dtype=torch.float16`) over the quant states the fused
+at every token count, differentiable in the input and every adapter's weights (DESIGN.md §6d).  DoRA adapters
+(`DoraAdapterSet`) train through `dora_linear4bit_group_multi` / `dora_linear4bit_multi` (DESIGN.md §6e).  The compute dtype is the base's (bf16, or fp16 for `compute_dtype=torch.float16`) over the quant states the fused
 path covers; the adapters are of it.
 """
 from __future__ import annotations
@@ -247,6 +248,7 @@ def lora_linear4bit_group_mixed(x: Tensor, bases, adapter_sets, adapter_names: U
     row of `x` (flattened to [M, K]) with its own adapter.  `adapter_names`: one name per row ("__base__": no adapter), as
     peft's `adapter_names`, or the int32 CUDA row-index tensor of `LoraAdapterSet.indices` (what a CUDA graph or a compiled
     graph takes; an index outside [0, len(set)) means no adapter).  Returns a tuple of outputs of x's shape[:-1] + [N]."""
+    _refuse_dora(adapter_sets)
     cdt = _validate(x, bases, adapter_sets)
     x2d = F.as_compute_2d(x, cdt)
     m = x2d.shape[0]
@@ -358,6 +360,7 @@ def lora_linear4bit_group_multi(x: Tensor, bases, adapter_sets, rows: Union[Sequ
 
     Every token count takes the segmented path, so no host branch depends on the indices and a step can be captured in a
     CUDA graph or compiled.  The gradients of the adapters' weights are views of one flat buffer per problem and kind."""
+    _refuse_dora(adapter_sets)
     cdt = _validate(x, bases, adapter_sets, training=True)
     if any(s.ranks != adapter_sets[0].ranks for s in adapter_sets):
         raise ValueError("grouped adapter sets must give each adapter the same rank")
@@ -376,3 +379,158 @@ def lora_linear4bit_multi(x: Tensor, base, adapter_set: LoraAdapterSet, rows: Un
                           x_lora: Tensor | None = None) -> Tensor:
     """`lora_linear4bit_group_multi` for one Linear4bit: `base(x)` plus each row's own adapter, trainable."""
     return lora_linear4bit_group_multi(x, [base], [adapter_set], rows, None if x_lora is None else [x_lora])[0]
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# training several DoRA adapters over one base in one batch (DESIGN.md §6e)
+# ----------------------------------------------------------------------------------------------------------------------
+
+class DoraAdapterSet(LoraAdapterSet):
+    """The DoRA adapters of one linear, `{name: (lora_A.weight [r, K], lora_B.weight [N, r], magnitude [N], scaling)}` (peft's
+    `use_dora=True`: the magnitude is `lora_magnitude_vector[name].weight`), built once.  `LoraAdapterSet`'s rules and
+    device tables, plus a device table of the magnitudes' addresses (of the adapters' dtype, contiguous, 16-byte aligned) and
+    the layouts of the stacked A rows and of the Gram matrices that the norms use.  The LoRA entry points refuse a
+    DoraAdapterSet: they would drop its magnitudes."""
+
+    def __init__(self, adapters: dict):
+        if not adapters:
+            raise ValueError("DoraAdapterSet: no adapters")
+        for name, entry in adapters.items():
+            if len(entry) != 4:
+                raise ValueError(f"adapter {name!r}: (lora_A.weight, lora_B.weight, magnitude, scaling)")
+        super().__init__({name: (a, b, s) for name, (a, b, _, s) in adapters.items()})
+        self.magnitudes = []
+        for name, (_, _, m, _) in adapters.items():
+            if (m.dim() != 1 or m.shape[0] != self.out_features or m.dtype != self.dtype or m.device != self.device
+                    or not m.is_contiguous() or m.data_ptr() % 16):
+                raise ValueError(f"adapter {name!r}: a contiguous, 16-byte aligned {self.dtype} magnitude "
+                                 f"[{self.out_features}] on {self.device}")
+            self.magnitudes.append(m)
+        self.mag_table = torch.tensor([m.data_ptr() for m in self.magnitudes], dtype=torch.int64).to(self.device)
+        ranks = torch.tensor(self.ranks, dtype=torch.int64)
+        # stacked row j of the norms' fused forward belongs to adapter stack_rows[j]; G_a sits at gram_offsets[a]
+        self.stack_rows = torch.arange(len(self.ranks), dtype=torch.int32).repeat_interleave(ranks).to(self.device)
+        sq = ranks * ranks
+        self.gram_total = int(sq.sum())
+        self.gram_offsets = (torch.cumsum(sq, 0) - sq).to(self.device)
+
+    def requires_grad(self) -> bool:
+        return super().requires_grad() or any(m.requires_grad for m in self.magnitudes)
+
+
+def _refuse_dora(sets) -> None:
+    if any(isinstance(s, DoraAdapterSet) for s in sets):
+        raise ValueError("a DoraAdapterSet holds magnitudes that the LoRA entry points would drop: use "
+                         "dora_linear4bit_group_multi / dora_linear4bit_multi")
+
+
+class MultiDoraMatMul4Bit(torch.autograd.Function):
+    """DoRA per row over n = 1..3 Linear4bit of one shape on one input (no bias): for row t with adapter a = rows[t] and
+    c_{p,a} = m_{p,a} / ||W_p + s B_{p,a} A_{p,a}||_row (detached, fp32),
+        no dropout  y_p[t] = c ⊙ (x[t] . W_p^T + U_p[t] . B_{p,a}^T)                       U_p[t] = rn(s . x[t] . A_{p,a}^T)
+        dropout     y_p[t] = x[t] . W_p^T + (c - 1) ⊙ (xd_p[t] . W_p^T) + c ⊙ U_p[t] . B_{p,a}^T   U from xd_p
+    and rows outside [0, n) take the base only.  Forward: the norms of every adapter (`dora_segmented_norm`), the base launch
+    (and with dropout the grouped launch on the dropped inputs), then the segmented shrink and DoRA expand
+    (`dora_segmented_fwd`).  Backward: `dora_grad_scale` (dQ, dD, dm), the base dX launches, then `dora_segmented_bwd`.
+    Differentiable in x, the dropped inputs and every adapter's A, B and magnitude."""
+
+    @staticmethod
+    def forward(ctx, x, rows, states, sets, n: int, *tensors):
+        x_loras, packeds = list(tensors[:n]), list(tensors[n:2 * n])
+        cdt = sets[0].dtype
+        x2d = F.as_compute_2d(x, cdt)
+        split = x_loras[0] is not None
+        xls = [F.as_compute_2d(t, cdt) for t in x_loras] if split else [x2d]
+        states = list(states)
+        n_ad, r = len(sets[0]), max(s.rmax for s in sets)
+        n_out, k_in = states[0].shape
+        sts = [F._state_tensors(qs, x2d.device) for qs in states]
+        norm2s = [F.weight_row_norm2(p, qs) for p, qs in zip(packeds, states)]
+        s0 = sets[0]
+        cs, nrms = _ops.dora_segmented_norm([s.table for s in sets], [s.mag_table for s in sets], s0.stack_rows, s0.rank_offsets,
+                                            s0.gram_offsets, s0.rank_total, s0.gram_total, packeds,
+                                            [a_f32 if a_u8 is None else a_u8 for a_u8, _, _, _, a_f32 in sts],
+                                            [t[1] for t in sts], [t[2] for t in sts], [t[3] for t in sts], n_out, k_in,
+                                            states[0].dtype, norm2s, cdt, n_ad, r)
+        outs = F.nf4_linear_group(False, [x2d] * n, packeds, states)
+        qs = F.nf4_linear_group(False, xls, packeds, states) if split else []
+        us, ws = _ops.dora_segmented_fwd(xls, [s.table for s in sets], rows, n_ad, r, cs, outs, qs)
+        ctx.save_for_backward(us, ws, cs, nrms, *xls, *packeds, *(qs if split else outs))
+        ctx.n, ctx.states, ctx.sets, ctx.r, ctx.split = n, states, sets, r, split
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.xl_meta = [(t.shape, t.dtype) for t in x_loras] if split else None
+        out_dtype = F.out_dtype_for(x.dtype, cdt)
+        return tuple((y if y.dtype == out_dtype else y.to(out_dtype)).view(*x.shape[:-1], n_out) for y in outs)
+
+    @staticmethod
+    def backward(ctx, *grad_ys):
+        n, sets, split = ctx.n, ctx.sets, ctx.split
+        us, ws, cs, nrms, *rest = ctx.saved_tensors
+        n_xl = n if split else 1
+        xls, packeds, qs = rest[:n_xl], rest[n_xl:n_xl + n], rest[n_xl + n:]
+        need = ctx.needs_input_grad
+        n_ad = len(sets[0])
+        cdt = sets[0].dtype
+        s0 = sets[0]
+        tables = [s.table for s in sets]
+        g2ds = [F.as_compute_2d(g, cdt) for g in grad_ys]
+        dq, dd, dm = _ops.dora_grad_scale(g2ds, tables, s0.rank_offsets, s0.rank_total, list(qs), cs, nrms, ws, n_ad, ctx.r, split)
+        if split:
+            dx = F.nf4_linear_group(True, g2ds, packeds, ctx.states, out_dtype=cdt) if need[0] else None
+            dxs = [F.nf4_linear_group(True, [dd[p]], [packeds[p]], [ctx.states[p]], out_dtype=cdt) for p in range(n)]
+        else:
+            dx = F.nf4_linear_group(True, list(dq.unbind(0)), packeds, ctx.states, out_dtype=cdt)
+            dxs = [dx]
+        d_a, d_b = _ops.dora_segmented_bwd(list(dq.unbind(0)), tables, s0.rank_offsets, s0.rank_total, us, list(xls), ws, n_ad,
+                                           ctx.r, dxs)
+        grad_x = None if dx is None or not need[0] else dx.to(ctx.x_dtype).view(ctx.x_shape)
+        grad_xls = [None] * n
+        if split:
+            for p in range(n):
+                if need[5 + p]:
+                    shape, dtype = ctx.xl_meta[p]
+                    grad_xls[p] = dxs[p].to(dtype).view(shape)
+        k, n_out = xls[0].shape[1], g2ds[0].shape[1]
+        offs, ranks = s0.rank_offsets_host, s0.ranks
+        base = 5 + 2 * n
+        grad_as = [d_a[p, offs[a] * k:(offs[a] + ranks[a]) * k].view(ranks[a], k) if need[base + p * n_ad + a] else None
+                   for p in range(n) for a in range(n_ad)]
+        base += n * n_ad
+        grad_bs = [d_b[p, offs[a] * n_out:(offs[a] + ranks[a]) * n_out].view(n_out, ranks[a]) if need[base + p * n_ad + a] else None
+                   for p in range(n) for a in range(n_ad)]
+        base += n * n_ad
+        grad_ms = [dm[p, a * n_out:(a + 1) * n_out] if need[base + p * n_ad + a] else None for p in range(n) for a in range(n_ad)]
+        return (grad_x, None, None, None, None, *grad_xls, *([None] * n), *grad_as, *grad_bs, *grad_ms)
+
+
+def dora_linear4bit_group_multi(x: Tensor, bases, dora_sets, rows: Union[Sequence[str], Tensor], x_loras=None):
+    """`lora_linear4bit_group_multi` for DoRA: `[per-row DoRA of dora_sets[p] over base_p]` for 1..3 Linear4bit of one
+    shape on one input (no bias), differentiable in `x`, in `x_loras` and in every adapter's lora_A, lora_B and magnitude
+    held by the `DoraAdapterSet`s, so one batch trains several QDoRA adapters over one frozen base.  `rows` and `x_loras`
+    as for `lora_linear4bit_group_multi`; the sets hold the same names with the same ranks.  Rows without an adapter
+    return `Linear4bit`'s bits.  No host branch depends on the indices or on device values, so a step can be captured in a
+    CUDA graph or compiled once the bases' row norms are cached (`functional.weight_row_norm2`).  The gradients of each
+    kind (A, B, magnitude) are views of one flat buffer per problem."""
+    if not all(isinstance(s, DoraAdapterSet) for s in dora_sets):
+        raise ValueError("dora_linear4bit_group_multi: one DoraAdapterSet per base")
+    cdt = _validate(x, bases, dora_sets, training=True)
+    if any(s.ranks != dora_sets[0].ranks for s in dora_sets):
+        raise ValueError("grouped adapter sets must give each adapter the same rank")
+    if any(b.bias is not None for b in bases):
+        raise ValueError("dora_linear4bit_group_multi: bases without bias")
+    n = len(bases)
+    if x_loras is not None:
+        if len(x_loras) != n or any(t.shape != x.shape or t.device != x.device for t in x_loras):
+            raise ValueError("x_loras: one input of x's shape per base")
+    m = x.numel() // x.shape[-1] if x.shape[-1] else 0
+    rows = _rows_tensor(rows, dora_sets, m, x.device)
+    tensors = [*(x_loras if x_loras is not None else [None] * n), *[b.weight.t() for b in bases],
+               *[a for s in dora_sets for a in s.lora_as], *[b for s in dora_sets for b in s.lora_bs],
+               *[mg for s in dora_sets for mg in s.magnitudes]]
+    return MultiDoraMatMul4Bit.apply(x, rows, tuple(b.weight.quant_state for b in bases), tuple(dora_sets), n, *tensors)
+
+
+def dora_linear4bit_multi(x: Tensor, base, dora_set: DoraAdapterSet, rows: Union[Sequence[str], Tensor],
+                          x_lora: Tensor | None = None) -> Tensor:
+    """`dora_linear4bit_group_multi` for one Linear4bit: each row's own DoRA adapter over `base`, trainable."""
+    return dora_linear4bit_group_multi(x, [base], [dora_set], rows, None if x_lora is None else [x_lora])[0]

@@ -19,6 +19,7 @@ from qlora_b200 import dora_linear4bit, dora_linear4bit_group, dora_linear4bit_p
 from qlora_b200 import LoraAdapterSet, lora_linear4bit_group_mixed, lora_linear4bit_mixed  # noqa: E402,F401
 # extensions: several adapters trained over one base in one batch
 from qlora_b200 import lora_linear4bit_group_multi, lora_linear4bit_multi  # noqa: E402,F401
+from qlora_b200 import DoraAdapterSet, dora_linear4bit_group_multi, dora_linear4bit_multi  # noqa: E402,F401
 from qlora_b200 import functional, nn, optim  # noqa: E402,F401
 
 __version__ = _impl.__version__
